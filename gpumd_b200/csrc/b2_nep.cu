@@ -6,6 +6,7 @@
 #include "b2_nep.cuh"
 #include "b2_nep_tc.cuh"
 #include "b2_nep_radial.cuh"
+#include "b2_nep_angular.cuh"
 #include "b2_nep_model.h"
 #include <cmath>
 #include <cstdlib>
@@ -341,6 +342,7 @@ struct b200md_nep {
   DevBuf<int> zbl_z;
   DevBuf<int> nn_r, nl_r, nn_a, nl_a;
   DevBuf<int> aslot, nla_rs; // see B2NepView::aslot
+  DevBuf<int> arev;          // few-type path: slot of i in the angular list of its m-th angular neighbour
   bool rev_slot = false;
   DevBuf<float> q, sfx, FpR, FpA, U, f12;
   DevBuf<double> acc;
@@ -491,17 +493,18 @@ int dispatch_force_final(
     const int4* p0 = p->nb.plane0.p;
     const int4* p1 = p->nb.plane1.p;
     const double* pz = p->nb.planez.p;
+    const int* ar = p->arev.p;
     // B200MD_NEP_VARIANT: resident blocks per SM the register allocation targets.  Measured on an
     // H100 (400 W) with 1 M-atom PbTe: 5 blocks / 96 regs 1.02 ms (default), 6 blocks / 80 regs with
     // spills 1.30 ms, 4 blocks / 128 regs (variant 2) 1.00 ms, variant 3 1.02 ms
 #define B2_FF2(NT_, ORTHO_)                                                                      \
   do {                                                                                           \
     if (p->variant == 1)                                                                         \
-      k_force_final2<NT_, K1, ORTHO_, 6><<<g, BLK, 0, st>>>(V, p0, p1, pz, box, pe, f, v);     \
+      k_force_final2<NT_, K1, ORTHO_, 6><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
     else if (p->variant == 2)                                                                    \
-      k_force_final2<NT_, K1, ORTHO_, 4><<<g, BLK, 0, st>>>(V, p0, p1, pz, box, pe, f, v);     \
+      k_force_final2<NT_, K1, ORTHO_, 4><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
     else                                                                                         \
-      k_force_final2<NT_, K1, ORTHO_, 5><<<g, BLK, 0, st>>>(V, p0, p1, pz, box, pe, f, v);     \
+      k_force_final2<NT_, K1, ORTHO_, 5><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
   } while (0)
     if (p->model.nt == 1 && box.ortho)
       B2_FF2(1, true);
@@ -523,9 +526,45 @@ int dispatch_force_final(
   return B200MD_OK;
 }
 
+// the few-type angular kernels of b2_nep_angular.cuh (with the plane-based radial passes)
+template <int NT, int K1, bool ORTHO>
+int launch_angular2(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool force)
+{
+  const int4* p0 = p->nb.plane0.p;
+  const int4* p1 = p->nb.plane1.p;
+  const double* pz = p->nb.planez.p;
+  const size_t ctab = (size_t)p->model.nt * p->model.nt * p->model.na1 * ((K1 + 3) / 4) * sizeof(float4);
+  if (!force) {
+    // + the per-thread staging of the angular descriptors when they go to the tile-major copy
+    const size_t qs = p->view.qt ? (size_t)p->model.dim_angular * BLK * sizeof(float) : 0;
+    auto dk = k_desc_angular2<NT, K1, 3, ORTHO>;
+    if (ctab + qs > 48 * 1024)
+      B2_CUDA(cudaFuncSetAttribute(dk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ctab + qs)));
+    dk<<<grid_for(p->n, BLK), BLK, ctab + qs, st>>>(p->view, p0, p1, pz, box);
+    B2_LAUNCHED();
+    return B200MD_OK;
+  }
+  auto kern = k_force_angular2<NT, K1, ORTHO>;
+  const size_t bytes = p->ang_smem + ctab;
+  if (bytes > 48 * 1024)
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  kern<<<grid_for(p->n, p->ang_block), p->ang_block, bytes, st>>>(p->view, p0, p1, pz, box, p->arev.p);
+  B2_LAUNCHED();
+  return B200MD_OK;
+}
+
 template <int K1>
 int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool force)
 {
+  if (p->radial_v2) {
+    if (p->model.nt == 1 && box.ortho)
+      return launch_angular2<1, K1, true>(p, box, st, force);
+    if (p->model.nt == 1)
+      return launch_angular2<1, K1, false>(p, box, st, force);
+    if (box.ortho)
+      return launch_angular2<2, K1, true>(p, box, st, force);
+    return launch_angular2<2, K1, false>(p, box, st, force);
+  }
   if (!force) {
     {
       // shared-memory copy of the angular coefficients when three blocks of it fit an SM
@@ -735,6 +774,8 @@ int nep_setup(b200md_nep* p, int num_atoms)
   B2_CUDA(p->FpA.reserve(N * m.dim_angular));
   B2_CUDA(p->U.reserve(N * m.UST));
   B2_CUDA(p->f12.reserve(N * 3 * m.MN_angular));
+  if (p->radial_v2)
+    B2_CUDA(p->arev.reserve(N * m.MN_angular));
   B2_CUDA(p->acc.reserve(N)); // site energies from the MLP pass
 
   B2NepView& P = p->view;
@@ -858,11 +899,13 @@ int nep_setup(b200md_nep* p, int num_atoms)
   }
 
   // shared-memory budgets
+  // (k_force_angular2: one padded row of b2_ang_ws4(na1) float4s per thread)
+  const size_t ang_row = p->radial_v2 ? b2_ang_ws4(m.na1) * sizeof(float4) : m.na1 * B2_NABC * sizeof(float);
   p->ang_block = BLK;
-  p->ang_smem = (size_t)m.na1 * B2_NABC * p->ang_block * sizeof(float);
+  p->ang_smem = ang_row * p->ang_block;
   while (p->ang_smem > 200 * 1024 && p->ang_block > 32) {
     p->ang_block /= 2;
-    p->ang_smem = (size_t)m.na1 * B2_NABC * p->ang_block * sizeof(float);
+    p->ang_smem = ang_row * p->ang_block;
   }
   // Radial descriptor of a many-type model: per-type accumulators in shared memory while two blocks of
   // them fit an SM, else (NEP89: 89 species) the per-pair contraction, which needs no such storage.
@@ -1056,7 +1099,7 @@ int b200md_nep_export_neighbors(
   if (d_NN_a && d_NL_a) {
     k_export_list<<<grid_for(n, 128), 128, 0, st>>>(
       n, p->rep_n ? p->rep_n : n, p->nb.perm.p, p->nn_a.p, p->nl_a.p, 1, (size_t)n, mn_a, d_NN_a,
-      d_NL_a, p->nb.flags.p, -1);
+      d_NL_a, p->nb.flags.p, p->radial_v2 ? B2_TAG_MASK : -1);
     B2_LAUNCHED();
   }
   return B200MD_OK;

@@ -46,6 +46,11 @@
 
 constexpr int B2_NABC = 24;      // (L_max+1)^2 - 1 for L_max = 4
 
+// list entry = neighbour index | type << 30 (B2NeighborView::tag_types; the radial and angular lists
+// of the few-type kernels in b2_nep_radial.cuh / b2_nep_angular.cuh)
+constexpr int B2_TAG_SHIFT = 30;
+constexpr int B2_TAG_MASK = (1 << B2_TAG_SHIFT) - 1;
+
 struct B2NepView {
   // ---- model (device tables) ----
   int nt;       // number of types
@@ -1237,7 +1242,7 @@ B2_HD void b2_zbl_sum(
   float pe = 0.0f, f[3] = {0.0f, 0.0f, 0.0f};
   float vxx = 0.0f, vyy = 0.0f, vzz = 0.0f, vxy = 0.0f, vxz = 0.0f, vyz = 0.0f;
   for (int m = m0; m < nn; m += mstep) {
-    const int j = P.nl_a[(size_t)m * N + i];
+    const int j = P.nl_a[(size_t)m * N + i] & B2_TAG_MASK; // the few-type path tags the entries
     const B2Atom a2 = b2_load_atom(&P.atoms[j]);
     float x12, y12, z12;
     b2_r12(geo, box, a1, a2, x12, y12, z12);

@@ -1,0 +1,410 @@
+// b2_nep_angular.cuh -- the two angular kernels of the NEP path for models with one or two atom types
+// (device only), on the layout of b2_nep_radial.cuh.  Same arithmetic per pair, op for op, as
+// b2_body_desc_angular / b2_body_force_angular in b2_nep.cuh (which tests/emu runs on the host and
+// which stay the many-type path); what differs is everything around the arithmetic:
+//   * neighbours come from the tagged angular list (index | type << B2_TAG_SHIFT, written by
+//     k_desc_radial2) and the {x,y} / z position planes: one 16-byte and one 8-byte gather per
+//     neighbour instead of a dependent 32-byte record;
+//   * the angular pair cutoffs of the <= 2 neighbour types live in registers, the minimum image of an
+//     orthogonal box is the branch-free one (b2_rec_r12);
+//   * the coefficient rows c_a4 are staged in shared memory once per block;
+//   * s[n][abc] travels between the two kernels as float4 planes sfx4[(n*6 + abc/4)*N + i]: the same
+//     480 bytes per atom (PbTe) with a quarter of the memory instructions;
+//   * the force kernel keeps the per-atom weights dU/ds[n][abc] in shared memory as ONE row per thread,
+//     read as float4s (the per-pair W / Wp contraction needs a quarter of the shared-memory loads);
+//   * the force kernel also finds, for each pair (i, j), the slot of i in j's angular list and stores
+//     it (arev), so that the pair reduction in k_force_final2 (b2_reduce_angular_planes) gathers f21
+//     directly instead of walking a binary search of dependent loads.
+#pragma once
+#include "b2_nep_radial.cuh"
+
+namespace b2 {
+
+constexpr int B2_ABC4 = B2_NABC / 4; // float4 groups of one angular channel
+
+// angular pair cutoffs of a type-t1 atom against neighbour types 0 .. NT-1, pinned in registers
+template <int NT>
+__device__ __forceinline__ void b2_ang_cutoffs(const B2NepView& P, int t1, float* rc, float* rcinv)
+{
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    const int pr = t1 * P.nt + (t < P.nt ? t : 0);
+    rc[t] = __ldg(&P.rc_a[pr]);
+    rcinv[t] = __ldg(&P.rcinv_a[pr]);
+    B2_PIN_F(rc[t]);
+    B2_PIN_F(rcinv[t]);
+  }
+}
+
+// every block copies the padded angular coefficients c_a4 ([nt*nt][na1][KQ] float4s, <= 2.9 KB with
+// two types) to shared memory; the caller syncs
+__device__ __forceinline__ void b2_stage_ctab(const B2NepView& P, float4* dst, int KQ)
+{
+  const int tot = P.nt * P.nt * P.na1 * KQ;
+  for (int e = threadIdx.x; e < tot; e += blockDim.x)
+    dst[e] = __ldg(&P.c_a4[e]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Angular descriptor.  The radial index n is processed in chunks of NCH channels so that the NCH*24
+// accumulators stay in registers; each chunk walks the (short) angular list once.  NCH = 3 at three
+// blocks per SM (146 registers for PbTe, no spills) measured faster on an H100 (400 W, 1 M-atom PbTe:
+// 0.41 ms) than one pass with NCH = 5 at two blocks per SM (198 registers, 0.48 ms); NCH = 5 at three
+// blocks spills.
+// ---------------------------------------------------------------------------------------------
+template <int NT, int K1, int NCH, bool ORTHO>
+__global__ void __launch_bounds__(128, 3) k_desc_angular2(
+  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
+  const double* __restrict__ pz, const B2Box box)
+{
+  static_assert(NT == 1 || NT == 2, "few-type path");
+  constexpr int KQ = (K1 + 3) / 4;
+  extern __shared__ float4 ctab_s[];
+  b2_stage_ctab(P, ctab_s, KQ);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const float C3B[B2_NABC] = {B2_C3B_LIST};
+  const B2GeoR geo = b2_geo_pinned(box);
+  const unsigned N = (unsigned)P.n;
+  const int na1 = P.na1;
+  const B2Rec a1 = b2_rec_load(p0, p1, i);
+  const int t1 = a1.t;
+  float rcv[NT], rciv[NT];
+  b2_ang_cutoffs<NT>(P, t1, rcv, rciv);
+  const float4* crow[NT]; // coefficient rows (t1, t2)
+#pragma unroll
+  for (int t = 0; t < NT; ++t)
+    crow[t] = ctab_s + (t1 * P.nt + (t < P.nt ? t : 0)) * na1 * KQ;
+  const int* __restrict__ list = P.nl_a;
+  const int nn = P.nn_a[i];
+  // descriptor component k of this atom: tile-major copy (k_mlp_tc) or SoA columns
+  float* const qb = P.qt ? P.qt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.q + i;
+  // With the tile-major copy the angular components are collected in shared memory (qs[(k-nr1)*128 + tid],
+  // after the coefficient table) and written once at the end as 16-byte groups: written where they are
+  // formed, one 4-byte store per component, the groups of a tile row would reach HBM as partial sectors
+  // in two passes over the list.
+  float* const qs = reinterpret_cast<float*>(ctab_s + P.nt * P.nt * na1 * KQ) + threadIdx.x;
+  auto qat = [&](int k) -> float* {
+    return P.qt ? qs + (size_t)(k - P.nr1) * 128 : qb + (size_t)k * N;
+  };
+  float4* __restrict__ sf4 = reinterpret_cast<float4*>(P.sfx);
+  for (int n0 = 0; n0 < na1; n0 += NCH) {
+    float s[NCH][B2_NABC];
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int abc = 0; abc < B2_NABC; ++abc)
+        s[c][abc] = 0.0f;
+    // list entries two neighbours ahead, positions one ahead
+    int e1 = nn > 1 ? __ldg(list + N + i) : i;
+    B2Rec rn = b2_rec_load_tagged(p0, pz, nn > 0 ? __ldg(list + i) : i);
+    for (int m = 0; m < nn; ++m) {
+      const B2Rec a2 = rn;
+      rn = b2_rec_load_tagged(p0, pz, e1);
+      e1 = (m + 2 < nn) ? __ldg(list + (unsigned)(m + 2) * N + i) : i;
+      float x12, y12, z12;
+      b2_rec_r12<ORTHO>(geo, box, a1, a2, x12, y12, z12);
+      const float d = sqrtf(b2_d2(x12, y12, z12));
+      const bool ty = NT > 1 && a2.t != 0;
+      float fn[K1];
+      b2_basis<K1>(d, ty ? rcv[NT - 1] : rcv[0], ty ? rciv[NT - 1] : rciv[0], fn);
+      const float dinv = 1.0f / d;
+      float B[B2_NABC];
+      b2_harmonics(x12 * dinv, y12 * dinv, z12 * dinv, B);
+      const float4* c4 = (ty ? crow[NT - 1] : crow[0]) + n0 * KQ;
+#pragma unroll
+      for (int c = 0; c < NCH; ++c) {
+        if (n0 + c < na1) {
+          float ck[KQ * 4];
+#pragma unroll
+          for (int q = 0; q < KQ; ++q) {
+            const float4 v = c4[c * KQ + q];
+            ck[4 * q] = v.x;
+            ck[4 * q + 1] = v.y;
+            ck[4 * q + 2] = v.z;
+            ck[4 * q + 3] = v.w;
+          }
+          float g = 0.0f;
+#pragma unroll
+          for (int k = 0; k < K1; ++k)
+            g = fmaf(fn[k], ck[k], g);
+#pragma unroll
+          for (int abc = 0; abc < B2_NABC; ++abc)
+            s[c][abc] = fmaf(g, B[abc], s[c][abc]);
+        }
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      const int n = n0 + c;
+      if (n < na1) {
+        // 3-body invariants, L = 1..4: q[nr1 + (L-1)*na1 + n]
+        int st = 0;
+#pragma unroll
+        for (int L = 1; L <= 4; ++L) {
+          float v = 0.0f;
+#pragma unroll
+          for (int k = 1; k < 2 * L + 1; ++k)
+            v = fmaf(C3B[st + k] * s[c][st + k], s[c][st + k], v);
+          v = 2.0f * v + C3B[st] * s[c][st] * s[c][st];
+          *qat(P.nr1 + (L - 1) * na1 + n) = v;
+          st += 2 * L + 1;
+        }
+        int Lidx = 4;
+        if (P.has222) {
+          const float* t = &s[c][3];
+          const float v = B2_C4B0 * t[0] * t[0] * t[0] + B2_C4B1 * t[0] * (t[1] * t[1] + t[2] * t[2]) +
+                          B2_C4B2 * t[0] * (t[3] * t[3] + t[4] * t[4]) +
+                          B2_C4B3 * t[3] * (t[2] * t[2] - t[1] * t[1]) + B2_C4B4 * t[1] * t[2] * t[4];
+          *qat(P.nr1 + Lidx * na1 + n) = v;
+          ++Lidx;
+        }
+        if (P.has1111) {
+          const float s0 = s[c][0] * s[c][0], tt = s[c][1] * s[c][1] + s[c][2] * s[c][2];
+          *qat(P.nr1 + Lidx * na1 + n) = B2_C5B0 * s0 * s0 + B2_C5B1 * s0 * tt + B2_C5B2 * tt * tt;
+        }
+#pragma unroll
+        for (int g = 0; g < B2_ABC4; ++g)
+          sf4[(size_t)(n * B2_ABC4 + g) * N + i] =
+            make_float4(s[c][4 * g], s[c][4 * g + 1], s[c][4 * g + 2], s[c][4 * g + 3]);
+      }
+    }
+  }
+  if (P.qt) {
+    const int klo = P.nr1, khi = P.dim;
+    for (int k0 = klo & ~3; k0 < khi; k0 += 4) {
+      float* dst = qb + (size_t)(k0 >> 2) * 512;
+      if (k0 >= klo && k0 + 4 <= khi) {
+        const float* src = qs + (size_t)(k0 - klo) * 128;
+        *reinterpret_cast<float4*>(dst) = make_float4(src[0], src[128], src[256], src[384]);
+      } else {
+        for (int r = 0; r < 4; ++r)
+          if (k0 + r >= klo && k0 + r < khi)
+            dst[r] = qs[(size_t)(k0 + r - klo) * 128];
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Angular partial forces f12 and the reverse slots arev.  Dynamic shared memory: blockDim.x rows of
+// WS4 = 6*na1 + 1 float4s (the per-atom weights; the odd row stride keeps the 128-bit accesses of a
+// quarter warp on distinct banks), then the coefficient table.
+// ---------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int b2_ang_ws4(int na1) { return B2_ABC4 * na1 + 1; }
+
+template <int NT, int K1, bool ORTHO>
+__global__ void __launch_bounds__(128, 3) k_force_angular2(
+  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
+  const double* __restrict__ pz, const B2Box box, int* __restrict__ arev)
+{
+  static_assert(NT == 1 || NT == 2, "few-type path");
+  constexpr int KQ = (K1 + 3) / 4;
+  extern __shared__ float4 fa_smem[];
+  const int na1 = P.na1;
+  const int WS4 = b2_ang_ws4(na1);
+  float4* const ctab_s = fa_smem + blockDim.x * WS4;
+  b2_stage_ctab(P, ctab_s, KQ);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const float C3B[B2_NABC] = {B2_C3B_LIST};
+  const unsigned N = (unsigned)P.n;
+  float4* const w = fa_smem + threadIdx.x * WS4;
+  // dU/dq of this atom: tile-major copy written by k_mlp_tc (component d at fbase + (d/4)*512 + d%4),
+  // or the SoA columns FpA[(d - nr1)*N + i] of the SIMT layer
+  const float* fbase = P.fpt ? P.fpt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.FpA + i;
+  auto FpAt = [&](int da) -> float { // da = index inside the angular part
+    if (P.fpt) {
+      const int d = P.nr1 + da;
+      return fbase[(size_t)(d >> 2) * 512 + (d & 3)];
+    }
+    return fbase[(size_t)da * N];
+  };
+  // ---- weights (as b2_body_force_angular) ----
+  const float4* __restrict__ sf4 = reinterpret_cast<const float4*>(P.sfx);
+  // the sums and dU/dq of NB channels are fetched together before any of them is used, so a warp waits
+  // for one memory latency per NB channels instead of one per channel (H100, 400 W, 1 M-atom PbTe:
+  // 0.42 ms with NB = 3 against 0.44 with NB = 1 and NB = 5; NB = 5 needs 168 registers and spills)
+  constexpr int NB = 3;
+  for (int n0 = 0; n0 < na1; n0 += NB) {
+    float4 sv[NB][B2_ABC4];
+    float Fv[NB][6];
+#pragma unroll
+    for (int c = 0; c < NB; ++c) {
+      const int n = n0 + c;
+      if (n < na1) {
+#pragma unroll
+        for (int g = 0; g < B2_ABC4; ++g)
+          sv[c][g] = sf4[(size_t)(n * B2_ABC4 + g) * N + i];
+#pragma unroll
+        for (int L = 0; L < 4; ++L)
+          Fv[c][L] = FpAt(L * na1 + n);
+        Fv[c][4] = P.has222 ? FpAt(4 * na1 + n) : 0.0f;
+        Fv[c][5] = P.has1111 ? FpAt((4 + (P.has222 ? 1 : 0)) * na1 + n) : 0.0f;
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < NB; ++c) {
+    const int n = n0 + c;
+    if (n >= na1)
+      break;
+    float s[B2_NABC];
+#pragma unroll
+    for (int g = 0; g < B2_ABC4; ++g) {
+      const float4 v = sv[c][g];
+      s[4 * g] = v.x;
+      s[4 * g + 1] = v.y;
+      s[4 * g + 2] = v.z;
+      s[4 * g + 3] = v.w;
+    }
+    float wv[B2_NABC];
+    int st = 0;
+#pragma unroll
+    for (int L = 1; L <= 4; ++L) {
+      const float F = Fv[c][L - 1];
+      wv[st] = 2.0f * F * C3B[st] * s[st];
+#pragma unroll
+      for (int k = 1; k < 2 * L + 1; ++k)
+        wv[st + k] = 4.0f * F * C3B[st + k] * s[st + k];
+      st += 2 * L + 1;
+    }
+    if (P.has222) {
+      const float F = Fv[c][4];
+      const float* t = &s[3];
+      wv[3] += F * (3.0f * B2_C4B0 * t[0] * t[0] + B2_C4B1 * (t[1] * t[1] + t[2] * t[2]) +
+                    B2_C4B2 * (t[3] * t[3] + t[4] * t[4]));
+      wv[4] += F * (2.0f * B2_C4B1 * t[0] * t[1] - 2.0f * B2_C4B3 * t[3] * t[1] + B2_C4B4 * t[2] * t[4]);
+      wv[5] += F * (2.0f * B2_C4B1 * t[0] * t[2] + 2.0f * B2_C4B3 * t[3] * t[2] + B2_C4B4 * t[1] * t[4]);
+      wv[6] += F * (2.0f * B2_C4B2 * t[0] * t[3] + B2_C4B3 * (t[2] * t[2] - t[1] * t[1]));
+      wv[7] += F * (2.0f * B2_C4B2 * t[0] * t[4] + B2_C4B4 * t[1] * t[2]);
+    }
+    if (P.has1111) {
+      const float F = Fv[c][5];
+      const float tt = s[1] * s[1] + s[2] * s[2];
+      wv[0] += F * (4.0f * B2_C5B0 * s[0] * s[0] * s[0] + 2.0f * B2_C5B1 * tt * s[0]);
+      wv[1] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[1] + 4.0f * B2_C5B2 * tt * s[1]);
+      wv[2] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[2] + 4.0f * B2_C5B2 * tt * s[2]);
+    }
+#pragma unroll
+    for (int g = 0; g < B2_ABC4; ++g)
+      w[n * B2_ABC4 + g] = make_float4(wv[4 * g], wv[4 * g + 1], wv[4 * g + 2], wv[4 * g + 3]);
+    }
+  }
+  // ---- pairs ----
+  const B2GeoR geo = b2_geo_pinned(box);
+  const B2Rec a1 = b2_rec_load(p0, p1, i);
+  const int t1 = a1.t;
+  float rcv[NT], rciv[NT];
+  b2_ang_cutoffs<NT>(P, t1, rcv, rciv);
+  const float4* crow[NT];
+#pragma unroll
+  for (int t = 0; t < NT; ++t)
+    crow[t] = ctab_s + (t1 * P.nt + (t < P.nt ? t : 0)) * na1 * KQ;
+  const int* __restrict__ list = P.nl_a;
+  const int* __restrict__ cnt = P.nn_a;
+  const int nn = cnt[i];
+  const size_t plane = (size_t)P.mn_a * N; // 3 planes may exceed 2^32 entries
+  // list entries two neighbours ahead; position and list length of the neighbour one ahead
+  int e1 = nn > 1 ? __ldg(list + N + i) : i;
+  int en = nn > 0 ? __ldg(list + i) : i;
+  B2Rec rn = b2_rec_load_tagged(p0, pz, en);
+  int cn = __ldg(&cnt[en & B2_TAG_MASK]);
+  for (int m = 0; m < nn; ++m) {
+    const B2Rec a2 = rn;
+    const int j = en & B2_TAG_MASK, cj = cn;
+    en = e1;
+    rn = b2_rec_load_tagged(p0, pz, en);
+    cn = __ldg(&cnt[en & B2_TAG_MASK]);
+    e1 = (m + 2 < nn) ? __ldg(list + (unsigned)(m + 2) * N + i) : i;
+    // slot of i in j's list: the number of j's neighbours below i (the list is a set); -> 0 when i is
+    // missing, as the binary search of b2_reduce_angular_sum.  Independent loads, issued before the
+    // pair arithmetic that hides them.
+    int below = 0, hit = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int v = q < cj ? (__ldg(list + (unsigned)q * N + j) & B2_TAG_MASK) : INT_MAX;
+      below += v < i ? 1 : 0;
+      hit |= v == i ? 1 : 0;
+    }
+    for (int q = 8; q < cj; ++q) {
+      const int v = __ldg(list + (unsigned)q * N + j) & B2_TAG_MASK;
+      below += v < i ? 1 : 0;
+      hit |= v == i ? 1 : 0;
+    }
+    float x12, y12, z12;
+    b2_rec_r12<ORTHO>(geo, box, a1, a2, x12, y12, z12);
+    const float d = sqrtf(b2_d2(x12, y12, z12));
+    const float dinv = 1.0f / d;
+    const bool ty = NT > 1 && a2.t != 0;
+    float fn[K1], fnp[K1];
+    b2_basis_d<K1, true>(d, ty ? rcv[NT - 1] : rcv[0], ty ? rciv[NT - 1] : rciv[0], fn, fnp);
+    float W[B2_NABC], Wp[B2_NABC];
+#pragma unroll
+    for (int abc = 0; abc < B2_NABC; ++abc) {
+      W[abc] = 0.0f;
+      Wp[abc] = 0.0f;
+    }
+    const float4* c4 = ty ? crow[NT - 1] : crow[0];
+    for (int n = 0; n < na1; ++n) {
+      float ck[KQ * 4];
+#pragma unroll
+      for (int q = 0; q < KQ; ++q) {
+        const float4 v = c4[n * KQ + q];
+        ck[4 * q] = v.x;
+        ck[4 * q + 1] = v.y;
+        ck[4 * q + 2] = v.z;
+        ck[4 * q + 3] = v.w;
+      }
+      float g = 0.0f, gp = 0.0f;
+#pragma unroll
+      for (int k = 0; k < K1; ++k) {
+        g = fmaf(fn[k], ck[k], g);
+        gp = fmaf(fnp[k], ck[k], gp);
+      }
+      const float4* wn = w + n * B2_ABC4;
+#pragma unroll
+      for (int q = 0; q < B2_ABC4; ++q) {
+        const float4 v = wn[q];
+        const float wq[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          W[4 * q + r] = fmaf(g, wq[r], W[4 * q + r]);
+          Wp[4 * q + r] = fmaf(gp, wq[r], Wp[4 * q + r]);
+        }
+      }
+    }
+    const float xh = x12 * dinv, yh = y12 * dinv, zh = z12 * dinv;
+    float B[B2_NABC];
+    b2_harmonics(xh, yh, zh, B);
+    // radial part: sum_abc (g' - L g / r) w b(rhat)
+    float ar = 0.0f, al = 0.0f;
+    {
+      int st = 0;
+#pragma unroll
+      for (int L = 1; L <= 4; ++L) {
+        float tl = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 2 * L + 1; ++k) {
+          ar = fmaf(Wp[st + k], B[st + k], ar);
+          tl = fmaf(W[st + k], B[st + k], tl);
+        }
+        al = fmaf((float)L, tl, al);
+        st += 2 * L + 1;
+      }
+    }
+    float gx, gy, gz;
+    b2_harmonics_grad_dot(xh, yh, zh, W, gx, gy, gz);
+    const float rad = ar - al * dinv;
+    const unsigned slot = (unsigned)m * N + i;
+    P.f12[slot] = fmaf(rad, xh, gx * dinv);
+    P.f12[plane + slot] = fmaf(rad, yh, gy * dinv);
+    P.f12[2 * plane + slot] = fmaf(rad, zh, gz * dinv);
+    arev[slot] = hit ? below : 0;
+  }
+}
+
+} // namespace b2
