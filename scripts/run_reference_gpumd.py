@@ -118,6 +118,17 @@ def main():
     d, i = run_case("sp_eam", s, ["Cu", "Fe", "Ni"], GOLDEN / "eam_zhou_2004_CuFeNi.txt", sp)
     collect_single_point(d, s, ["Cu", "Fe", "Ni"]); infos.append(i)
 
+    # one- and two-species synthetic models (tests/golden/make_synthetic_models.py) on the features NEP_CPU
+    # cannot pin: typewise ZBL, per-species cutoffs, and NEP5 with flexible ZBL.  fcc a = 3.1 A with the two
+    # species drawn i.i.d., 2048 atoms, 24.8 A box
+    for name, model in (("sp_typewise_zbl", "nep_synth_2sp_typewise_zbl.txt"),
+                        ("sp_pertype_cut", "nep_synth_2sp_pertype_cut.txt"),
+                        ("sp_nep5_flexzbl", "nep_synth_2sp_nep5_flexzbl.txt")):
+        sym = nep_type_order(GOLDEN / model)
+        s = fcc(8, 3.1, rattle=0.15, seed=61, num_types=2, symbols=("Ar", "Ar"))
+        d, i = run_case(name, s, sym, GOLDEN / model, sp)
+        collect_single_point(d, s, sym); infos.append(i)
+
     # ---- (2) NVE trajectories from given velocities: thermo.out every 10 steps ----
     md = "ensemble nve\ntime_step {dt}\ndump_thermo 10\nrun {steps}\n"
     s = rocksalt_pbte(20, rattle=0.02, seed=1)  # 64 000 atoms

@@ -5,7 +5,7 @@ Everything copied here is DATA the reference's own tests/examples pin this path 
 No reference source code is copied.  /root/reference does not exist on the GPU box, so the
 tests only ever read the committed copies.
 
-    python tests/golden/make_fixtures.py
+    python tests/golden/make_fixtures.py [few_species]
 """
 import gzip
 import shutil
@@ -79,6 +79,7 @@ def main():
                         pos_r=(e11 - q * 10**7).astype(np.int32))
     print("wrote carbon_model.npz", pos.shape)
     nep_cpu_goldens()
+    nep_cpu_goldens_few_species()
 
 
 def nep_cpu_goldens():
@@ -100,5 +101,26 @@ def nep_cpu_goldens():
     print("wrote ref_nep_cpu.npz", sorted(out))
 
 
+def nep_cpu_goldens_few_species():
+    """The same for the synthetic one- and two-species models NEP_CPU reads (NEP5, flexible and universal
+    ZBL): inputs of tests/test_few_species_cpu.py::test_oracle_matches_reference_nep_cpu_few_species."""
+    root = OUT.parents[1]
+    sys.path[:0] = [str(root), str(root / "tests")]
+    from oracle import oracle_py
+    from test_few_species_cpu import NEP_CPU_FEW_SPECIES, nep_cpu_few_species_structure
+    assert oracle_py.ref_available(), "oracle/_ref/libnep_cpu_ref.so not built"
+    out = {}
+    for case, model in NEP_CPU_FEW_SPECIES.items():
+        s = nep_cpu_few_species_structure(model)
+        r = oracle_py.RefNepCpu(OUT / model).compute(s["type"], s["h"], s["pos"])
+        for k in ("pe", "force", "virial"):
+            out[f"{case}_{k}"] = np.asarray(r[k], dtype=np.float64)
+    np.savez_compressed(OUT / "ref_nep_cpu_few_species.npz", **out)
+    print("wrote ref_nep_cpu_few_species.npz", sorted(out))
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["few_species"]:  # only the NEP_CPU results of the synthetic few-species models
+        nep_cpu_goldens_few_species()
+    else:
+        main()
