@@ -129,8 +129,36 @@ def main():
         d, i = run_case(name, s, sym, GOLDEN / model, sp)
         collect_single_point(d, s, sym); infos.append(i)
 
+    # LJ / Tersoff / EAM beyond one orthogonal, periodic, few-species crystal (tests/cases_classical.py):
+    # per-pair LJ tables in a triclinic box, the Tersoff SiC mixing rules (also with an open direction),
+    # Dai-2006, and the power/log embedding branch of Zhou-2004 Cu (a = 3.3 A)
+    sys.path.insert(0, str(ROOT / "tests"))
+    from cases import shear, slab
+    from cases_classical import _sic
+    lj3 = ["Ar", "Ne", "Kr"]
+    s = shear(fcc(8, 5.30, rattle=0.1, seed=62, num_types=3, symbols=("Ar", "Ar", "Ar")))  # 2048 atoms
+    d, i = run_case("sp_lj3_tric", s, lj3, GOLDEN / "lj_synth_3types.txt", sp)
+    collect_single_point(d, s, lj3); infos.append(i)
+    for name, s in (("sp_sic", _sic(6, 63)), ("sp_sic_slab", slab(_sic(6, 64)))):  # 1728 atoms, 26.2 A
+        d, i = run_case(name, s, ["Si", "C"], GOLDEN / "tersoff_SiC_1989.txt", sp)
+        collect_single_point(d, s, ["Si", "C"]); infos.append(i)
+    s = fcc(8, 3.615, rattle=0.08, seed=65, symbols=("Cu",))  # 2048 atoms
+    d, i = run_case("sp_eam_dai", s, ["Cu"], GOLDEN / "eam_Cu_Dai_2006.txt", sp)
+    collect_single_point(d, s, ["Cu"]); infos.append(i)
+    s = fcc(8, 3.3, rattle=0.08, seed=66, symbols=("Cu",))
+    d, i = run_case("sp_eam_cu_compressed", s, ["Cu"], GOLDEN / "eam_Cu_Zhou_2004.txt", sp)
+    collect_single_point(d, s, ["Cu"]); infos.append(i)
+    s = shear(fcc(8, 3.615, rattle=0.08, seed=67, num_types=3, symbols=["Cu", "Fe", "Ni"]))
+    d, i = run_case("sp_eam_alloy_tric", s, ["Cu", "Fe", "Ni"], GOLDEN / "eam_zhou_2004_CuFeNi.txt", sp)
+    collect_single_point(d, s, ["Cu", "Fe", "Ni"]); infos.append(i)
+
     # ---- (2) NVE trajectories from given velocities: thermo.out every 10 steps ----
     md = "ensemble nve\ntime_step {dt}\ndump_thermo 10\nrun {steps}\n"
+    s = fcc(10, 3.615, rattle=0.0, seed=1, num_types=3, symbols=["Cu", "Fe", "Ni"])  # 4000 atoms
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    d, i = run_case("md_eam", s, ["Cu", "Fe", "Ni"], GOLDEN / "eam_zhou_2004_CuFeNi.txt",
+                    md.format(dt=1, steps=200), vel)
+    infos.append(i)
     s = rocksalt_pbte(20, rattle=0.02, seed=1)  # 64 000 atoms
     vel = init_velocities(s["mass"], 300.0, seed=42)
     d, i = run_case("md_pbte", s, pbte_sym, GOLDEN / "nep_PbTe.txt", md.format(dt=1, steps=200), vel)
