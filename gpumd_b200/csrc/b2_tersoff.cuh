@@ -198,15 +198,25 @@ B2_HD void b2_body_tersoff_reduce(int i, const B2TersoffView& P, const B2Box& bo
   acc[12 * N] = v[7];
 }
 
-// per-atom heat current (gpu_compute_heat, src/measure/compute_heat.cu:32-63)
+// per-atom heat current jx_in jx_out jy_in jy_out jz (gpu_compute_heat,
+// src/measure/compute_heat.cu:32-63).  The one definition of these expressions: compute_heat / HAC
+// (b2_body_heat) and the fused HNEMD heat sum (b2_measure.cu) both call it.
+B2_HD void b2_heat5(int i, int stride, const double* w, const double* vel, double h[5])
+{
+  const size_t n = (size_t)stride;
+  const double vx = vel[i], vy = vel[n + i], vz = vel[2 * n + i];
+  h[0] = w[i] * vx + w[3 * n + i] * vy;
+  h[1] = w[4 * n + i] * vz;
+  h[2] = w[6 * n + i] * vx + w[n + i] * vy;
+  h[3] = w[5 * n + i] * vz;
+  h[4] = w[7 * n + i] * vx + w[8 * n + i] * vy + w[2 * n + i] * vz;
+}
+
 B2_HD void b2_body_heat(
   int i, int stride, const double* w, const double* vel, double* heat, int hstride)
 {
-  const size_t n = (size_t)stride, hn = (size_t)hstride;
-  const double vx = vel[i], vy = vel[n + i], vz = vel[2 * n + i];
-  heat[i] = w[i] * vx + w[3 * n + i] * vy;
-  heat[hn + i] = w[4 * n + i] * vz;
-  heat[2 * hn + i] = w[6 * n + i] * vx + w[n + i] * vy;
-  heat[3 * hn + i] = w[5 * n + i] * vz;
-  heat[4 * hn + i] = w[7 * n + i] * vx + w[8 * n + i] * vy + w[2 * n + i] * vz;
+  double h[5];
+  b2_heat5(i, stride, w, vel, h);
+  for (int k = 0; k < 5; ++k)
+    heat[(size_t)hstride * k + i] = h[k];
 }

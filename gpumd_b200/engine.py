@@ -364,6 +364,14 @@ class Force:
             self._zero = False
         return pot
 
+    _fe = None
+
+    def set_hnemd(self, fe):
+        """compute_hnemd's driving force (Force::set_hnemd_parameters, force.cu:341-360): every following
+        compute() adds W_i^T fe to each force and removes the net force.  fe = None switches it off
+        (Force::finalize, force.cu:335-339)."""
+        self._fe = None if fe is None else (C.c_double * 3)(*[float(x) for x in fe])
+
     def compute(self, box, position, type_, potential, force, virial):
         n = type_.shape[0]
         st = _stream()
@@ -371,6 +379,100 @@ class Force:
         if self._zero:
             _lib.check(self._L.b200md_zero_properties(n, _ptr(potential), _ptr(force), _ptr(virial), st))
         self.potentials[0].compute(box, type_, position, potential, force, virial)
+        if self._fe is not None:
+            hnemd_drive(n, self._fe, virial, force)
+
+
+_drive_scratch = {}
+
+
+def hnemd_drive(n, fe, virial, force):
+    """b200md_hnemd_drive on device arrays: force += W^T fe per atom, then the net force is removed
+    (force.cu:857-897).  fe: 3 floats (1/A)."""
+    L = _lib.load()
+    dev = force.device
+    need = int(L.b200md_hnemd_drive_scratch_bytes(int(n)))
+    s = _drive_scratch.get(dev)
+    if s is None or s.numel() < need:
+        s = torch.zeros(need, dtype=torch.uint8, device=dev)  # the ticket starts at zero
+        _drive_scratch[dev] = s
+    fe3 = fe if isinstance(fe, C.Array) else (C.c_double * 3)(*[float(x) for x in fe])
+    _lib.check(L.b200md_hnemd_drive(int(n), int(n), fe3, _ptr(virial), _ptr(force), _ptr(s), _stream()))
+
+
+class HNEMD:
+    """compute_hnemd, src/measure/hnemd_kappa.cu: process(step, atom) every step; take() after every
+    output_interval-th step returns kappa[5] (W/mK: xx_in xx_out yy_in yy_out zz) and the heat sums
+    rows[output_interval, 5] of the finished interval."""
+
+    def __init__(self, output_interval, fe):
+        _require_cuda()
+        self._L = _lib.load()
+        self.output_interval = int(output_interval)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_hnemd_create(self.output_interval, (C.c_double * 3)(*[float(x) for x in fe]),
+                                               C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.b200md_hnemd_destroy(self._h)
+            self._h = None
+
+    def process(self, step, atom):
+        n = atom.number_of_atoms
+        _lib.check(self._L.b200md_hnemd_sample(self._h, int(step), n, n, _ptr(atom.virial_per_atom),
+                                               _ptr(atom.velocity_per_atom), _stream()))
+
+    def take(self, volume, temperature):
+        kappa, rows = np.zeros(5), np.zeros(5 * self.output_interval)
+        dp = C.POINTER(C.c_double)
+        _lib.check(self._L.b200md_hnemd_take(self._h, float(volume), float(temperature), kappa.ctypes.data_as(dp),
+                                             rows.ctypes.data_as(dp), _stream()))
+        return kappa, rows.reshape(self.output_interval, 5)
+
+
+class SHC:
+    """compute_shc, src/measure/shc.cu.  groups: None for the whole system of num_atoms atoms, or a
+    list of int arrays, the atom indices of each output group (Group::find_contents order).
+    process(step, atom) every step; postprocess() returns ki, ko [num_groups, 2Nc-1] and shc_i, shc_o
+    [num_groups, num_omega]."""
+
+    def __init__(self, sample_interval, Nc, direction, number_of_steps, num_atoms=None, groups=None):
+        _require_cuda()
+        self._L = _lib.load()
+        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
+        if groups is None:
+            sizes, contents = np.array([int(num_atoms)], np.int32), None
+        else:
+            sizes = np.array([len(g) for g in groups], np.int32)
+            contents = np.ascontiguousarray(np.concatenate([np.asarray(g, np.int32) for g in groups]))
+        self.num_groups = sizes.shape[0]
+        ip = C.POINTER(C.c_int)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_shc_create(
+            self.Nc, self.sample_interval, int(direction), int(number_of_steps), self.num_groups,
+            sizes.ctypes.data_as(ip), None if contents is None else contents.ctypes.data_as(ip), C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.b200md_shc_destroy(self._h)
+            self._h = None
+
+    def process(self, step, atom):
+        n = atom.number_of_atoms
+        _lib.check(self._L.b200md_shc_sample(self._h, int(step), n, n, _ptr(atom.virial_per_atom),
+                                             _ptr(atom.velocity_per_atom), _stream()))
+
+    def postprocess(self, time_step, num_omega, max_omega):
+        g, nk, nw = self.num_groups, 2 * self.Nc - 1, int(num_omega)
+        ki, ko, si, so = np.zeros(g * nk), np.zeros(g * nk), np.zeros(max(g * nw, 1)), np.zeros(max(g * nw, 1))
+        dp = C.POINTER(C.c_double)
+        _lib.check(self._L.b200md_shc_finish(
+            self._h, float(time_step), nw, float(max_omega), ki.ctypes.data_as(dp), ko.ctypes.data_as(dp),
+            si.ctypes.data_as(dp), so.ctypes.data_as(dp), _stream()))
+        return ki.reshape(g, nk), ko.reshape(g, nk), si[:g * nw].reshape(g, nw), so[:g * nw].reshape(g, nw)
 
 
 class Ensemble_NVE:

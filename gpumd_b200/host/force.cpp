@@ -53,4 +53,19 @@ void Force::compute(
     b2h_fail("Force::compute (zero)");
   potentials[0]->compute(
     box, type, position_per_atom, potential_per_atom, force_per_atom, virial_per_atom);
+  if (hnemd_) { // force.cu:857-897, after the potential has stored or accumulated its outputs
+    const size_t need = (size_t)b200md_hnemd_drive_scratch_bytes(n);
+    if (drive_scratch_.size() < need)
+      drive_scratch_.resize(need, 0); // the ticket starts at zero
+    if (b200md_hnemd_drive(n, n, fe_, virial_per_atom.data(), force_per_atom.data(),
+                           drive_scratch_.data(), nullptr) != B200MD_OK)
+      b2h_fail("Force::compute (HNEMD driving force)");
+  }
+}
+
+void Force::set_hnemd(const double fe[3])
+{
+  hnemd_ = true;
+  for (int d = 0; d < 3; ++d)
+    fe_[d] = fe[d];
 }

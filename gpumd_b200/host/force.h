@@ -15,8 +15,16 @@ public:
     Box& box, GPU_Vector<double>& position_per_atom, GPU_Vector<int>& type,
     GPU_Vector<double>& potential_per_atom, GPU_Vector<double>& force_per_atom,
     GPU_Vector<double>& virial_per_atom);
+  // compute_hnemd (Force::set_hnemd_parameters, force.cu:341-360): every following compute adds the
+  // driving force W_i^T fe and removes the net force; finalize() switches it off again after a run
+  // (Force::finalize, force.cu:335-339)
+  void set_hnemd(const double fe[3]);
+  void finalize() { hnemd_ = false; }
   std::vector<std::unique_ptr<Potential>> potentials;
 
 private:
   bool zero_first_ = true; // false when the single potential overwrites its outputs (NEP_B200)
+  bool hnemd_ = false;
+  double fe_[3] = {0.0, 0.0, 0.0};
+  GPU_Vector<char> drive_scratch_; // b200md_hnemd_drive_scratch_bytes, allocated once
 };

@@ -48,6 +48,9 @@ public:
   int number = 0;             // number of groups of this grouping method
   std::vector<int> cpu_label; // group label of every atom (group.cuh:25)
   std::vector<int> cpu_size;  // atoms per group
+  std::vector<int> cpu_size_sum; // atoms in the groups before each group (group.cu:50-56)
+  std::vector<int> contents;  // atom indices sorted by group, then by index (Group::find_contents,
+                              // group.cu:58-70)
   GPU_Vector<int> label;      // device copy of cpu_label
 };
 

@@ -13,13 +13,14 @@
 //   Replicate                                       src/main_gpumd/replicate.cu:20-111
 // Keywords: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
 // nvt_ber|nvt_nhc|nvt_bdp T T tau, time_step <fs>, dump_thermo <n>, dump_xyz <n> <file> [precision
-// single|double] [mass velocity force potential virial], dump_restart <n>, run <n>.  Anything else is an
-// input error (exit 1), as in the reference.
+// single|double] [mass velocity force potential virial], dump_restart <n>, compute_hac, compute_hnemd,
+// compute_shc, run <n>.  Anything else is an input error (exit 1), as in the reference.
 #include "ensemble.h"
 #include "force.h"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <fstream>
 #include <map>
@@ -46,6 +47,27 @@ static bool element_mass(const std::string& symbol, double* mass)
 {
   fprintf(stderr, "Input Error:\n    %s\n", msg.c_str());
   exit(1);
+}
+
+// is_valid_int / is_valid_real, src/utilities/read_file.cu: the whole token must be the number
+static bool valid_int(const std::string& s, int* v)
+{
+  char* end = nullptr;
+  const long x = std::strtol(s.c_str(), &end, 10);
+  if (s.empty() || *end != '\0' || x < -2147483647L || x > 2147483647L)
+    return false;
+  *v = (int)x;
+  return true;
+}
+
+static bool valid_real(const std::string& s, double* v)
+{
+  char* end = nullptr;
+  const double x = std::strtod(s.c_str(), &end);
+  if (s.empty() || *end != '\0')
+    return false;
+  *v = x;
+  return true;
 }
 
 static std::string lower(std::string s)
@@ -183,6 +205,13 @@ static void read_model(const char* path, Model& m)
     g.cpu_size.assign(g.number, 0);
     for (int n = 0; n < N; ++n)
       g.cpu_size[g.cpu_label[n]]++;
+    g.cpu_size_sum.assign(g.number, 0);
+    for (int k = 1; k < g.number; ++k)
+      g.cpu_size_sum[k] = g.cpu_size_sum[k - 1] + g.cpu_size[k - 1];
+    g.contents.assign(N, 0);
+    std::vector<int> fill(g.cpu_size_sum);
+    for (int n = 0; n < N; ++n)
+      g.contents[fill[g.cpu_label[n]]++] = n;
     g.label.resize(N);
     g.label.copy_from_host(g.cpu_label.data());
   }
@@ -332,6 +361,18 @@ private:
   struct HacSpec {
     int interval = 0, Nc = 0, output_interval = 1;
   } hac_spec_;
+  // compute_hnemd output_interval fe_x fe_y fe_z (hnemd_kappa.cu:142-184) and compute_shc
+  // sample_interval Nc direction num_omega max_omega [group method id] (shc.cu:466-542); both are
+  // reset after each run (HNEMD::postprocess, SHC::postprocess, Force::finalize)
+  struct HnemdSpec {
+    int output_interval = 0; // 0: off
+    double fe[3] = {0.0, 0.0, 0.0};
+  } hnemd_spec_;
+  struct ShcSpec {
+    int sample_interval = 0; // 0: off
+    int Nc = 0, direction = 0, num_omega = 0, group_method = -1, group_id = 0;
+    double max_omega = 0.0;
+  } shc_spec_;
   double global_time_ = 0.0; // natural units, as Run::global_time (run.cu:316)
   bool state_on_gpu_ = false;
   bool has_potential_ = false;
@@ -515,6 +556,10 @@ private:
         input_error("compute_hac parameters should be positive integers.");
       printf("Compute HAC.\n    sample interval is %d.\n    Nc is %d\n    output_interval is %d\n",
              hac_spec_.interval, hac_spec_.Nc, hac_spec_.output_interval);
+    } else if (t[0] == "compute_hnemd") {
+      parse_compute_hnemd(t);
+    } else if (t[0] == "compute_shc") {
+      parse_compute_shc(t);
     } else if (t[0] == "dump_restart") {
       if (t.size() != 2 || std::atoi(t[1].c_str()) <= 0)
         input_error("dump_restart should have 1 positive parameter (the interval).");
@@ -532,12 +577,139 @@ private:
       fixed_group_ = move_group_ = -1;
       fixed_method_ = move_method_ = 0;
       hac_spec_ = HacSpec();
+      hnemd_spec_ = HnemdSpec();
+      shc_spec_ = ShcSpec();
+      force_.finalize();
       dump_thermo_ = 0; // non-propagating keywords are reset after each run (run.cu:329-340)
       dump_restart_ = 0;
       dump_xyz_ = XyzDump();
     } else {
       input_error("'" + t[0] + "' is not a keyword supported by the b200md backend.");
     }
+  }
+
+  void parse_compute_hnemd(const std::vector<std::string>& t)
+  {
+    printf("Compute thermal conductivity using the HNEMD method.\n");
+    if (t.size() != 5)
+      input_error("compute_hnemd should have 4 parameters.");
+    HnemdSpec h;
+    if (!valid_int(t[1], &h.output_interval))
+      input_error("output_interval for HNEMD should be an integer number.");
+    if (h.output_interval < 1)
+      input_error("output_interval for HNEMD should be larger than 0.");
+    const char* names[3] = {"fe_x", "fe_y", "fe_z"};
+    for (int d = 0; d < 3; ++d)
+      if (!valid_real(t[2 + d], &h.fe[d]))
+        input_error(std::string(names[d]) + " for HNEMD should be a real number.");
+    if (hnemd_spec_.output_interval > 0) // Force::set_hnemd_parameters, force.cu:344-346
+      input_error("Cannot have more than one HNEMD method within one run.");
+    printf("    output_interval = %d\n    fe = (%g, %g, %g) /A\n", h.output_interval, h.fe[0], h.fe[1],
+           h.fe[2]);
+    hnemd_spec_ = h;
+    force_.set_hnemd(h.fe); // already in force for the evaluation before the loop (run.cu:217-248)
+  }
+
+  void parse_compute_shc(const std::vector<std::string>& t)
+  {
+    printf("Compute SHC.\n");
+    if (t.size() != 6 && t.size() != 9)
+      input_error("compute_shc should have 5 or 8 parameters.");
+    ShcSpec c;
+    if (!valid_int(t[1], &c.sample_interval))
+      input_error("Sampling interval for SHC should be an integer.");
+    if (c.sample_interval < 1)
+      input_error("Sampling interval for SHC should >= 1.");
+    if (c.sample_interval > 50)
+      input_error("Sampling interval for SHC should <= 50 (trust me).");
+    if (!valid_int(t[2], &c.Nc))
+      input_error("Nc for SHC should be an integer.");
+    if (c.Nc < 100)
+      input_error("Nc for SHC should >= 100 (trust me).");
+    if (c.Nc > 1000)
+      input_error("Nc for SHC should <= 1000 (trust me).");
+    if (!valid_int(t[3], &c.direction))
+      input_error("direction for SHC should be an integer.");
+    if (c.direction < 0 || c.direction > 2)
+      input_error("Transport direction should be x or y or z.");
+    if (!valid_int(t[4], &c.num_omega))
+      input_error("num_omega for SHC should be an integer.");
+    if (c.num_omega < 0)
+      input_error("num_omega for SHC should >= 0.");
+    if (!valid_real(t[5], &c.max_omega))
+      input_error("max_omega for SHC should be a number.");
+    if (c.max_omega <= 0)
+      input_error("max_omega for SHC should > 0.");
+    if (t.size() == 9) { // parse_group(..., allow_all_groups = true), parse_utilities.cu:27-60
+      if (t[6] != "group")
+        input_error("Unrecognized argument in compute_shc.");
+      if (!valid_int(t[7], &c.group_method))
+        input_error("Grouping method should be an integer.");
+      if (c.group_method < 0)
+        input_error("Grouping method should >= 0.");
+      if (c.group_method >= (int)model_.group.size())
+        input_error("Grouping method should < number of grouping methods.");
+      if (!valid_int(t[8], &c.group_id))
+        input_error("Group ID should be an integer.");
+      if (c.group_id >= model_.group[c.group_method].number)
+        input_error("Group ID should < number of groups.");
+      if (c.group_id < -1)
+        input_error("group ID should >= -1 for computing SHC.");
+      if (c.group_id == -1 && model_.group[c.group_method].number < 2)
+        input_error("compute_shc with group ID -1 needs a grouping method with at least two groups.");
+    }
+    printf("    sampling interval %d, Nc %d, direction %d, num_omega %d, max_omega %g\n",
+           c.sample_interval, c.Nc, c.direction, c.num_omega, c.max_omega);
+    shc_spec_ = c;
+  }
+
+  // SHC::postprocess, shc.cu:398-464: header, then per output group 2Nc-1 correlation rows and
+  // num_omega spectrum rows
+  void write_shc(b200md_shc* shc, int num_groups)
+  {
+    const ShcSpec& c = shc_spec_;
+    const int Nk = 2 * c.Nc - 1;
+    std::vector<double> ki((size_t)num_groups * Nk), ko(ki.size());
+    std::vector<double> si((size_t)num_groups * c.num_omega + 1), so(si.size());
+    if (b200md_shc_finish(shc, time_step_, c.num_omega, c.max_omega, ki.data(), ko.data(), si.data(),
+                          so.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute_shc");
+    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
+    const double d_omega = c.max_omega / c.num_omega;
+    FILE* fid = fopen("shc.out", "a");
+    if (!fid)
+      input_error("Failed to open shc.out.");
+    fprintf(fid, "# compute_shc %d %d %d %d %g", c.sample_interval, c.Nc, c.direction, c.num_omega,
+            c.max_omega);
+    if (c.group_method >= 0)
+      fprintf(fid, " group %d %d", c.group_method, c.group_id);
+    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n", model_.atom.number_of_atoms);
+    const double* h = model_.box.cpu_h;
+    fprintf(fid, "# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6],
+            h[1], h[4], h[7], h[2], h[5], h[8]);
+    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
+    fprintf(fid, "# num_correlation_rows %d\n", Nk);
+    fprintf(fid, "# num_frequency_rows %d\n", c.num_omega);
+    if (c.group_method >= 0 && c.group_id == -1)
+      fprintf(fid, "# num_output_groups %d\n", num_groups);
+    fprintf(fid, "# columns_correlation time_ps ki ko\n");
+    fprintf(fid, "# columns_shc omega_THz shc_i shc_o\n");
+    for (int g = 0; g < num_groups; ++g) {
+      for (int nc = 0; nc < Nk; ++nc) // ki, ko in A eV/ps
+        fprintf(fid, "%g %g %g\n", (nc + 1 - c.Nc) * dt_in_ps, ki[(size_t)g * Nk + nc],
+                ko[(size_t)g * Nk + nc]);
+      for (int nw = 0; nw < c.num_omega; ++nw) // shc_i, shc_o in A eV = A eV/ps/THz
+        fprintf(fid, "%g %g %g\n", (nw + 1) * d_omega, si[(size_t)g * c.num_omega + nw],
+                so[(size_t)g * c.num_omega + nw]);
+    }
+    fclose(fid);
+  }
+
+  // the temperature the measurements use: run.cu passes integrate.temperature2, which an nve line
+  // leaves at the last thermostatted value
+  double measure_temperature() const
+  {
+    return ensemble_spec_.type == 0 ? hac_temperature_ : ensemble_spec_.T;
   }
 
   // Replicate: copies ordered a-slowest, c-fastest, atoms innermost; box columns scaled
@@ -807,6 +979,31 @@ private:
       if (b200md_hac_create(number_of_steps, hac_spec_.interval, hac_spec_.Nc, &hac) != B200MD_OK)
         input_error(std::string("compute_hac: ") + b200md_last_error());
     }
+    b200md_hnemd* hnemd = nullptr;
+    if (hnemd_spec_.output_interval > 0 &&
+        b200md_hnemd_create(hnemd_spec_.output_interval, hnemd_spec_.fe, &hnemd) != B200MD_OK)
+      b2h_fail("compute_hnemd");
+    b200md_shc* shc = nullptr;
+    int shc_groups = 1;
+    if (shc_spec_.sample_interval > 0) {
+      const ShcSpec& c = shc_spec_;
+      std::vector<int> sizes(1, a.number_of_atoms);
+      const int* contents = nullptr; // the whole system in atom order
+      if (c.group_method >= 0) {
+        const Group& g = model_.group[c.group_method];
+        const int first = c.group_id == -1 ? 1 : c.group_id; // id -1: every group except 0
+        const int last = c.group_id == -1 ? g.number - 1 : c.group_id;
+        sizes.assign(g.cpu_size.begin() + first, g.cpu_size.begin() + last + 1);
+        contents = g.contents.data() + g.cpu_size_sum[first]; // the groups are contiguous there
+      }
+      shc_groups = (int)sizes.size();
+      const int rc = b200md_shc_create(c.Nc, c.sample_interval, c.direction, number_of_steps, shc_groups,
+                                       sizes.data(), contents, &shc);
+      if (rc == B200MD_ERR_ARG)
+        input_error(std::string("compute_shc: ") + b200md_last_error());
+      if (rc != B200MD_OK)
+        b2h_fail("compute_shc");
+    }
     printf("Run %d steps.\n", number_of_steps);
     const auto t0 = std::chrono::high_resolution_clock::now();
     for (int step = 0; step < number_of_steps; ++step) {
@@ -817,6 +1014,28 @@ private:
       if (hac && b200md_hac_sample(hac, step, a.number_of_atoms, a.number_of_atoms,
                                    a.virial_per_atom.data(), a.velocity_per_atom.data(), nullptr) != B200MD_OK)
         b2h_fail("compute_hac");
+      if (hnemd) {
+        if (b200md_hnemd_sample(hnemd, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
+                                a.velocity_per_atom.data(), nullptr) != B200MD_OK)
+          b2h_fail("compute_hnemd");
+        if ((step + 1) % hnemd_spec_.output_interval == 0) { // hnemd_kappa.cu:108-131
+          force_.potentials[0]->check();
+          double kappa[5];
+          if (b200md_hnemd_take(hnemd, model_.box.get_volume(), measure_temperature(), kappa, nullptr,
+                                nullptr) != B200MD_OK)
+            b2h_fail("compute_hnemd");
+          FILE* fk = fopen("kappa.out", "a");
+          if (!fk)
+            input_error("Failed to open kappa.out.");
+          for (int k = 0; k < 5; ++k)
+            fprintf(fk, "%25.15f", kappa[k]);
+          fprintf(fk, "\n");
+          fclose(fk);
+        }
+      }
+      if (shc && b200md_shc_sample(shc, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
+                                   a.velocity_per_atom.data(), nullptr) != B200MD_OK)
+        b2h_fail("compute_shc");
       ++global_step_;
       global_time_ += time_step_;
       const bool out_thermo = fid && (step + 1) % dump_thermo_ == 0;
@@ -842,8 +1061,8 @@ private:
     if (hac) { // HAC::postprocess, hac.cu:186-258: hac.out = t(ps), 5 hac averages, 5 rtc averages
       const int Nc = hac_spec_.Nc, oi = hac_spec_.output_interval;
       std::vector<double> h((size_t)5 * Nc), r((size_t)5 * Nc);
-      if (b200md_hac_finish(hac, time_step_, ensemble_spec_.type == 0 ? hac_temperature_ : ensemble_spec_.T,
-                            model_.box.get_volume(), h.data(), r.data(), nullptr) != B200MD_OK)
+      if (b200md_hac_finish(hac, time_step_, measure_temperature(), model_.box.get_volume(), h.data(),
+                            r.data(), nullptr) != B200MD_OK)
         b2h_fail("compute_hac");
       const double dt_in_ps = time_step_ * hac_spec_.interval * TIME_UNIT_CONVERSION / 1000.0;
       FILE* fh = fopen("hac.out", "a");
@@ -861,6 +1080,12 @@ private:
       }
       fclose(fh);
       b200md_hac_destroy(hac);
+    }
+    if (hnemd)
+      b200md_hnemd_destroy(hnemd);
+    if (shc) {
+      write_shc(shc, shc_groups);
+      b200md_shc_destroy(shc);
     }
   }
 };

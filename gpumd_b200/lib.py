@@ -80,6 +80,16 @@ SIGNATURES = {
     "b200md_hac_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200md_hac_finish": (C.c_int, [_vp, C.c_double, C.c_double, C.c_double, _dp, _dp, _vp]),
     "b200md_hac_series": (C.c_int, [_vp, _dp, _vp]),
+    "b200md_hnemd_drive_scratch_bytes": (C.c_longlong, [C.c_int]),
+    "b200md_hnemd_drive": (C.c_int, [C.c_int, C.c_int, _dp, _vp, _vp, _vp, _vp]),
+    "b200md_hnemd_create": (C.c_int, [C.c_int, _dp, C.POINTER(_vp)]),
+    "b200md_hnemd_destroy": (None, [_vp]),
+    "b200md_hnemd_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "b200md_hnemd_take": (C.c_int, [_vp, C.c_double, C.c_double, _dp, _dp, _vp]),
+    "b200md_shc_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _ip, _ip, C.POINTER(_vp)]),
+    "b200md_shc_destroy": (None, [_vp]),
+    "b200md_shc_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "b200md_shc_finish": (C.c_int, [_vp, C.c_double, C.c_int, C.c_double, _dp, _dp, _dp, _dp, _vp]),
     "b200md_langevin_create": (C.c_int, [C.c_int, C.c_ulonglong, C.POINTER(_vp)]),
     "b200md_langevin_destroy": (None, [_vp]),
     "b200md_langevin_apply": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_double, _vp, _vp, _vp]),

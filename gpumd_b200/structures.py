@@ -71,7 +71,8 @@ def read_xyz(path, type_order=None):
 
 
 def write_xyz(path, s, symbols, vel=None):
-    """model.xyz in GPUMD's dialect; vel (natural units) is written in A/fs (read_xyz.cu:380-387)."""
+    """model.xyz in GPUMD's dialect; vel (natural units) is written in A/fs (read_xyz.cu:380-387).
+    s["group"] (optional, int [N]): one grouping method, written as group:I:1 (read_xyz.cu:271-287)."""
     n = s["type"].shape[0]
     h = np.asarray(s["h"], dtype=np.float64).reshape(3, 3)
     lat = " ".join(f"{v:.17g}" for v in h.T.reshape(-1))  # lattice= lists a, b, c
@@ -82,6 +83,9 @@ def write_xyz(path, s, symbols, vel=None):
     if vel is not None:
         v = np.asarray(vel) / TIME_UNIT_CONVERSION
         cols += [v[0], v[1], v[2]]
+    if s.get("group") is not None:
+        props += ":group:I:1"
+        cols.append(np.asarray(s["group"], dtype=np.int64))
     sym = np.asarray(symbols)[s["type"]]
     with open(path, "w") as f:
         f.write(f"{n}\n")
@@ -167,6 +171,25 @@ def diamond(reps, a=5.431, rattle=0.0, seed=1, symbol="Si"):
     s["mass"] = np.full(pos.shape[0], MASS[symbol])
     return s
 
+
+
+def graphene_sheet(nx=100, ny=101):
+    """The sheet of the reference's graphene HNEMD case (tests/gpumd/graphene_kappa_hnemd/create_xyz.m):
+    4-atom rectangular cell (a = 1.42 sqrt 3, b = 4.26, c = 3.35 A), nx x ny x 1 cells, pbc T T F, and
+    one grouping method of 9 slabs along y (cell rows 0 | 1-20 | 21-30 | ... | 71-80 | 81-)."""
+    r0 = np.array([[0.5, 0, 0], [0, 1 / 6, 0], [0, 0.5, 0], [0.5, 2 / 3, 0]])
+    a = np.array([1.42 * np.sqrt(3), 1.42 * 3, 3.35])
+    pos, label = [], []
+    for j in range(ny):
+        for i in range(nx):
+            for m in range(4):
+                pos.append(a * (np.array([i, j, 0]) + r0[m]))
+                label.append(0 if j == 0 else 1 if j <= 20 else min(2 + (j - 21) // 10, 8))
+    pos = np.array(pos)
+    n = pos.shape[0]
+    return dict(pos=np.ascontiguousarray(pos.T), type=np.zeros(n, np.int32),
+                h=np.diag(a * np.array([nx, ny, 1])).reshape(9), pbc=np.array([1, 1, 0], np.int32),
+                group=np.array(label, np.int32), mass=np.full(n, MASS["C"]), symbols=["C"])
 
 
 def init_velocities(mass, temperature, seed=42):

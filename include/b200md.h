@@ -246,6 +246,64 @@ int b200md_hac_finish(
   double* rtc_out, void* stream);
 int b200md_hac_series(b200md_hac* p, double* out, void* stream);
 
+/* Homogeneous non-equilibrium MD (HNEMD) thermal conductivity, the rest of SURVEY.md 8f rank 4.
+ *   b200md_hnemd_drive   <- Force::compute's compute_hnemd_ branch, src/force/force.cu:857-897 with
+ *                           gpu_add_driving_force / gpu_sum_force / gpu_correct_force (:228-312):
+ *                           f_i += W_i^T fe (virial map 0 3 4 / 6 1 5 / 7 8 2), then f_i -= sum_j f_j / n.
+ *                           The per-atom add is the reference's bit for bit; only the order of the
+ *                           total-force sum differs (fixed, so deterministic).  fe[3] (host) in 1/A;
+ *                           d_scratch: b200md_hnemd_drive_scratch_bytes(n) bytes of device memory,
+ *                           zeroed before the first call (no allocation per step; the reference
+ *                           allocates ftot at every step, force.cu:880)
+ *   b200md_hnemd_create  <- HNEMD::parse / preprocess, hnemd_kappa.cu:37-50, 149-184 (fe[3] host)
+ *   b200md_hnemd_sample  <- HNEMD::process, :82-106: call every step; the heat current of all atoms
+ *                           (compute_heat.cu:32-90) is summed straight into row step % output_interval
+ *                           of a device buffer, without the 5N per-atom array
+ *   b200md_hnemd_take    <- the output branch of HNEMD::process, :108-131: copies the finished interval
+ *                           to the host (the only copy) and writes kappa5[k] = sum of the rows *
+ *                           1.573769e5 / output_interval / (volume * temperature * |fe|) in W/mK, k =
+ *                           xx_in xx_out yy_in yy_out zz; rows (may be NULL) gets the 5*output_interval
+ *                           heat sums [m*5 + k] */
+long long b200md_hnemd_drive_scratch_bytes(int n);
+int b200md_hnemd_drive(
+  int n, int stride, const double fe[3], const double* d_virial, double* d_force, void* d_scratch,
+  void* stream);
+typedef struct b200md_hnemd b200md_hnemd;
+int b200md_hnemd_create(int output_interval, const double fe[3], b200md_hnemd** out);
+void b200md_hnemd_destroy(b200md_hnemd* p);
+int b200md_hnemd_sample(
+  b200md_hnemd* p, int step, int n, int stride, const double* d_virial, const double* d_velocity,
+  void* stream);
+int b200md_hnemd_take(
+  b200md_hnemd* p, double volume, double temperature, double* kappa5, double* rows, void* stream);
+
+/* Spectral heat current (SHC).  Replaces SHC::parse / preprocess / process / postprocess
+ * (src/measure/shc.cu:34-542):
+ *   b200md_shc_create  <- parse (:466-542) + preprocess (:34-79).  Output groups: num_groups sizes and
+ *                         (host) contents, the atom indices of group 0, then group 1, ... (concatenated
+ *                         in Group::find_contents order, group.cu:58-70).  contents = NULL: one group,
+ *                         the atoms 0 .. group_sizes[0]-1 (no grouping).  `group m -1` passes groups
+ *                         1 .. number-1 of method m.  Checks 1 <= sample_interval <= 50, 100 <= Nc <=
+ *                         1000, direction 0..2, and that number_of_steps gives at least one time origin.
+ *                         B200MD_ERR_CUDA when the device ring does not fit.
+ *   b200md_shc_sample  <- process (:162-310): call every step.  Every sample_interval steps the virial
+ *                         row of `direction` and the velocities of the groups go into a device ring;
+ *                         the correlation is deferred and computed for blocks of time origins
+ *   b200md_shc_finish  <- average_k + find_shc (:312-396), FP64 on the host: ki / ko [num_groups *
+ *                         (2Nc-1)] (Hann-windowed, A eV/ps) and shc_i / shc_o [num_groups * num_omega]
+ *                         (A eV), host arrays; time_step in natural units, max_omega in THz rad */
+typedef struct b200md_shc b200md_shc;
+int b200md_shc_create(
+  int Nc, int sample_interval, int direction, int number_of_steps, int num_groups,
+  const int* group_sizes, const int* contents, b200md_shc** out);
+void b200md_shc_destroy(b200md_shc* p);
+int b200md_shc_sample(
+  b200md_shc* p, int step, int n, int stride, const double* d_virial, const double* d_velocity,
+  void* stream);
+int b200md_shc_finish(
+  b200md_shc* p, double time_step, int num_omega, double max_omega, double* ki, double* ko,
+  double* shc_i, double* shc_o, void* stream);
+
 /* Langevin thermostats and the Berendsen barostat (SURVEY.md 8f rank 3):
  *   b200md_langevin_*         <- curand states + gpu_langevin + momentum correction,
  *                                src/integrate/langevin_utilities.cuh:26-127; one apply() = one

@@ -197,6 +197,23 @@ def main():
                     vel)
     infos.append(i)
 
+    # HNEMD + SHC: the sheet of the reference's own graphene_kappa_hnemd case (FP64 Tersoff), shortened,
+    # and PbTe NEP (FP32 force path) with SHC over every group but 0 of four slabs along x
+    from gpumd_b200.structures import graphene_sheet
+    s = graphene_sheet()  # 40 400 atoms, 9 groups along y
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    d, i = run_case("hnemd_graphene", s, ["C"], GOLDEN / "Graphene_Lindsay_2010_modified.txt",
+                    "ensemble nvt_nhc 300 300 100\ntime_step 1\ndump_thermo 10\ncompute_hnemd 20 0 0.00001 0\n"
+                    "compute_shc 1 100 1 200 400.0 group 0 4\nrun 400\n", vel)
+    infos.append(i)
+    s = rocksalt_pbte(12, rattle=0.02, seed=31)  # 13 824 atoms
+    s["group"] = np.minimum((s["pos"][0] / s["h"][0] * 4).astype(np.int32), 3)
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    d, i = run_case("hnemd_pbte", s, pbte_sym, GOLDEN / "nep_PbTe.txt",
+                    "ensemble nvt_ber 300 300 100\ntime_step 1\ndump_thermo 10\ncompute_hnemd 10 0.00002 0 0\n"
+                    "compute_shc 2 100 0 100 200 group 0 -1\nrun 250\n", vel)
+    infos.append(i)
+
     # ---- (3) throughput at the BASELINE sizes ----
     if not args.skip_speed:
         s = rocksalt_pbte(50, rattle=0.02, seed=1)  # C3: 1 000 000 atoms
