@@ -82,6 +82,44 @@ B2_HD void b2_body_vv_groups(
   b2_body_vv(i, stride, step1, dt, mass, pos, vel, f);
 }
 
+// Nose-Hoover chain of length 4, Suzuki-Yoshida order 7 x 4 RESPA sub-steps (the `nhc` function of
+// src/integrate/ensemble_nhc.cu:101-171, after Tuckerman) over half a time step.  state = {eta[4],
+// v_eta[4], Q[4]}; ek2 = twice the kinetic energy the chain couples to, dof its degrees of freedom.
+// Returns the velocity scale factor.  Shared by nvt_nhc and the two chains of heat_nhc.
+B2_HD double b2_nhc_chain(double* state, double ek2, double dof, double kT, double dt_half)
+{
+  constexpr int M = 4;
+  const double w[7] = {0.784513610477560, 0.235573213359357, -1.17767998417887, 1.31518632068391,
+                       -1.17767998417887, 0.235573213359357, 0.784513610477560};
+  double* eta = state;
+  double* ve = state + M;
+  const double* Q = state + 2 * M;
+  double factor = 1.0;
+  for (int a = 0; a < 7; ++a) {
+    const double dt2 = dt_half * w[a] / 4.0, dt4 = 0.5 * dt2, dt8 = 0.5 * dt4;
+    for (int b = 0; b < 4; ++b) {
+      ve[M - 1] += dt4 * (ve[M - 2] * ve[M - 2] / Q[M - 2] - kT);
+      for (int m = M - 2; m >= 0; --m) {
+        const double damp = exp(-dt8 * ve[m + 1] / Q[m + 1]);
+        const double G = (m == 0) ? ek2 - dof * kT : ve[m - 1] * ve[m - 1] / Q[m - 1] - kT;
+        ve[m] = damp * (damp * ve[m] + dt4 * G);
+      }
+      for (int m = M - 1; m >= 0; --m)
+        eta[m] += dt2 * ve[m] / Q[m];
+      const double f = exp(-dt2 * ve[0] / Q[0]);
+      ek2 *= f * f;
+      factor *= f;
+      for (int m = 0; m < M - 1; ++m) {
+        const double damp = exp(-dt8 * ve[m + 1] / Q[m + 1]);
+        const double G = (m == 0) ? ek2 - dof * kT : ve[m - 1] * ve[m - 1] / Q[m - 1] - kT;
+        ve[m] = damp * (damp * ve[m] + dt4 * G);
+      }
+      ve[M - 1] += dt4 * (ve[M - 2] * ve[M - 2] / Q[M - 2] - kT);
+    }
+  }
+  return factor;
+}
+
 // per-atom contributions to the 8 sums: m v^2, U, W_ab + m v_a v_b (ab = xx,yy,zz,xy,xz,yz)
 B2_HD void b2_thermo_terms(
   int i, int stride, const double* mass, const double* pe, const double* vel, const double* virial,

@@ -123,44 +123,14 @@ __global__ void __launch_bounds__(BLK) k_berendsen(
   }
 }
 
-// Nose-Hoover chain of length 4, Suzuki-Yoshida order 7 x 4 RESPA sub-steps (the scheme of
-// ensemble_nhc.cu:101-171, after Tuckerman); state = {eta[4], v_eta[4], Q[4], factor}.
+// Nose-Hoover chain (b2_nhc_chain); state = {eta[4], v_eta[4], Q[4], factor}.
 __global__ void k_nhc_chain(
   double* state, const double* __restrict__ thermo, double dof, double kT, double dt_half)
 {
   if (threadIdx.x != 0 || blockIdx.x != 0)
     return;
-  constexpr int M = 4;
-  const double w[7] = {0.784513610477560, 0.235573213359357, -1.17767998417887, 1.31518632068391,
-                       -1.17767998417887, 0.235573213359357, 0.784513610477560};
-  double* eta = state;
-  double* ve = state + M;
-  const double* Q = state + 2 * M;
-  double ek2 = thermo[0] * dof * 8.617343e-5; // 2 x kinetic energy from the instantaneous T
-  double factor = 1.0;
-  for (int a = 0; a < 7; ++a) {
-    const double dt2 = dt_half * w[a] / 4.0, dt4 = 0.5 * dt2, dt8 = 0.5 * dt4;
-    for (int b = 0; b < 4; ++b) {
-      ve[M - 1] += dt4 * (ve[M - 2] * ve[M - 2] / Q[M - 2] - kT);
-      for (int m = M - 2; m >= 0; --m) {
-        const double damp = exp(-dt8 * ve[m + 1] / Q[m + 1]);
-        const double G = (m == 0) ? ek2 - dof * kT : ve[m - 1] * ve[m - 1] / Q[m - 1] - kT;
-        ve[m] = damp * (damp * ve[m] + dt4 * G);
-      }
-      for (int m = M - 1; m >= 0; --m)
-        eta[m] += dt2 * ve[m] / Q[m];
-      const double f = exp(-dt2 * ve[0] / Q[0]);
-      ek2 *= f * f;
-      factor *= f;
-      for (int m = 0; m < M - 1; ++m) {
-        const double damp = exp(-dt8 * ve[m + 1] / Q[m + 1]);
-        const double G = (m == 0) ? ek2 - dof * kT : ve[m - 1] * ve[m - 1] / Q[m - 1] - kT;
-        ve[m] = damp * (damp * ve[m] + dt4 * G);
-      }
-      ve[M - 1] += dt4 * (ve[M - 2] * ve[M - 2] / Q[M - 2] - kT);
-    }
-  }
-  state[3 * M] = factor;
+  const double ek2 = thermo[0] * dof * 8.617343e-5; // 2 x kinetic energy from the instantaneous T
+  state[12] = b2_nhc_chain(state, ek2, dof, kT, dt_half);
 }
 
 __global__ void k_bdp_seed(B2BdpState* state, unsigned seed)

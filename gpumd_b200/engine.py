@@ -695,5 +695,164 @@ class Ensemble_NHC(Ensemble_NVE):
         self._thermostat(time_step, box, atom, thermo)
 
 
+def _group_contents(label):
+    """Group::find_contents (group.cu:50-70) of a label array: sizes[g], atom indices by group."""
+    lab = np.asarray(label.cpu() if torch.is_tensor(label) else label, dtype=np.int64).reshape(-1)
+    sizes = np.bincount(lab).astype(np.int32) if lab.size else np.zeros(1, np.int32)
+    contents = np.ascontiguousarray(np.argsort(lab, kind="stable").astype(np.int32))
+    return sizes, contents
+
+
+class _Ensemble_HEAT(Ensemble_NVE):
+    """Direct NEMD with a heat source and a heat sink (groups of grouping method 0, `label`):
+    the bath acts before velocity-Verlet step 1 and after step 2; no thermo is computed, as in the
+    reference.  energy_transferred() synchronises and returns the energy (eV) moved from the system
+    into the source and sink baths so far."""
+    KIND = -1
+
+    def __init__(self, label, source, sink, temperature, temperature_coupling, delta_temperature,
+                 time_step, seed_source=0, seed_sink=0):
+        lab = np.asarray(label.cpu() if torch.is_tensor(label) else label, dtype=np.int32).reshape(-1)
+        super().__init__(lab.shape[0])
+        self._label = torch.as_tensor(lab, device="cuda")
+        sizes, contents = _group_contents(lab)
+        ip = C.POINTER(C.c_int)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_heat_bath_create(
+            self.KIND, lab.shape[0], sizes.shape[0], sizes.ctypes.data_as(ip), contents.ctypes.data_as(ip),
+            int(source), int(sink), float(temperature), float(temperature_coupling), float(delta_temperature),
+            float(time_step), int(seed_source), int(seed_sink), C.byref(h)))
+        self._bath = h
+
+    def __del__(self):
+        if getattr(self, "_bath", None):
+            self._L.b200md_heat_bath_destroy(self._bath)
+            self._bath = None
+
+    def set_groups(self, label=None, fixed_group=-1, move_group=-1, move_velocity=(0.0, 0.0, 0.0)):
+        """fix / move on grouping method 0 (the label given at construction when label is None).  Only
+        heat_lan allows a moving group (integrate.cu:69)."""
+        if int(move_group) >= 0 and self.KIND != 0:
+            raise ValueError("It is only allowed to use nvt_ber, nvt_nhc, or nvt_bdp with a moving group.")
+        super().set_groups(self._label if label is None else label, fixed_group, move_group, move_velocity)
+
+    def half(self, after_vv2, atom):
+        n = atom.number_of_atoms
+        _lib.check(self._L.b200md_heat_bath_half(self._bath, int(after_vv2), n, n, _ptr(atom.mass),
+                                                 _ptr(atom.velocity_per_atom), _stream()))
+
+    def compute1(self, time_step, box, atom, thermo=None):
+        self.half(0, atom)
+        self._vv(1, time_step, atom)
+
+    def compute2(self, time_step, box, atom, thermo=None):
+        self._vv(0, time_step, atom)
+        self.half(1, atom)
+
+    def energy_transferred(self):
+        out = np.zeros(2)
+        _lib.check(self._L.b200md_heat_bath_energy(self._bath, out.ctypes.data_as(C.POINTER(C.c_double)),
+                                                   _stream()))
+        return out
+
+    def state(self):
+        """dict of the device record: chain[2,12], stat[2,5], vc[2,3], factor[2], energy[2]."""
+        out = np.zeros(44)
+        _lib.check(self._L.b200md_heat_bath_state(self._bath, out.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  _stream()))
+        return {"chain": out[:24].reshape(2, 12), "stat": out[24:34].reshape(2, 5),
+                "vc": out[34:40].reshape(2, 3), "factor": out[40:42], "energy": out[42:44]}
+
+
+class Ensemble_HEAT_LAN(_Ensemble_HEAT):
+    """heat_lan (type 22), ensemble_lan.cu:43-85,128-269: local Langevin half kicks on source and sink.
+    seed_source / seed_sink: the reference's first and second rand() (1804289383, 846930886 under its
+    -DDEBUG build)."""
+    KIND = 0
+
+    def __init__(self, label, source, sink, temperature, temperature_coupling, delta_temperature,
+                 time_step=1.0 / TIME_UNIT_CONVERSION, seed_source=1804289383, seed_sink=846930886):
+        super().__init__(label, source, sink, temperature, temperature_coupling, delta_temperature,
+                         time_step, seed_source, seed_sink)
+
+
+class Ensemble_HEAT_NHC(_Ensemble_HEAT):
+    """heat_nhc (type 21), ensemble_nhc.cu:52-91,239-326: two Nose-Hoover chains on the relative
+    kinetic energies of source and sink, scaling about each group's centre of mass."""
+    KIND = 1
+
+    def __init__(self, label, source, sink, temperature, temperature_coupling, delta_temperature, time_step):
+        super().__init__(label, source, sink, temperature, temperature_coupling, delta_temperature, time_step)
+
+
+class Ensemble_HEAT_BDP(_Ensemble_HEAT):
+    """heat_bdp (type 23), ensemble_bdp.cu:50-62,103-149: stochastic velocity rescaling of source then
+    sink after step 2, one MT19937 stream (seed 12345678 = the reference's -DDEBUG seed)."""
+    KIND = 2
+
+    def __init__(self, label, source, sink, temperature, temperature_coupling, delta_temperature,
+                 time_step=1.0 / TIME_UNIT_CONVERSION, seed=12345678):
+        super().__init__(label, source, sink, temperature, temperature_coupling, delta_temperature,
+                         time_step, seed, 0)
+
+
+COMPUTE_QUANTITIES = ("temperature", "potential", "force", "virial", "jp", "jk", "momentum")
+COMPUTE_WIDTH = (1, 1, 3, 9, 3, 3, 3)
+
+
+class Compute:
+    """`compute`, src/measure/compute.cu: group sums of the selected quantities over grouping method
+    `label`, sampled every sample_interval steps and averaged over output_interval samples.
+    process(step, atom) every step returns None, or on an output step the averages as an array
+    [columns, num_groups] in the reference's column order (temperature per atom)."""
+
+    def __init__(self, label, sample_interval, output_interval, quantities):
+        _require_cuda()
+        self._L = _lib.load()
+        mask = 0
+        for q in quantities:
+            if q not in COMPUTE_QUANTITIES:
+                raise ValueError(f"Invalid property for compute: {q}")
+            mask |= 1 << COMPUTE_QUANTITIES.index(q)
+        self.sizes, contents = _group_contents(label)
+        self.num_atoms = int(np.asarray(label.cpu() if torch.is_tensor(label) else label).reshape(-1).shape[0])
+        self.num_groups = int(self.sizes.shape[0])
+        self.sample_interval, self.output_interval = int(sample_interval), int(output_interval)
+        ip = C.POINTER(C.c_int)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_group_compute_create(self.num_atoms, self.num_groups,
+                                                       self.sizes.ctypes.data_as(ip),
+                                                       contents.ctypes.data_as(ip), mask, C.byref(h)))
+        self._h = h
+        self.num_columns = self._L.b200md_group_compute_columns(h)
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.b200md_group_compute_destroy(self._h)
+            self._h = None
+
+    def sample(self, atom):
+        n = atom.number_of_atoms
+        _lib.check(self._L.b200md_group_compute_sample(
+            self._h, n, n, _ptr(atom.mass), _ptr(atom.potential_per_atom), _ptr(atom.force_per_atom),
+            _ptr(atom.virial_per_atom), _ptr(atom.velocity_per_atom), _stream()))
+
+    def take(self, num_samples=None):
+        out = np.zeros(self.num_columns * self.num_groups)
+        _lib.check(self._L.b200md_group_compute_take(
+            self._h, int(num_samples or self.output_interval), out.ctypes.data_as(C.POINTER(C.c_double)),
+            _stream()))
+        return out.reshape(self.num_columns, self.num_groups)
+
+    def process(self, step, atom):
+        """Compute::process, compute.cu:351-538."""
+        if (step + 1) % self.sample_interval != 0:
+            return None
+        self.sample(atom)
+        if ((step + 1) // self.sample_interval) % self.output_interval == 0:
+            return self.take()
+        return None
+
+
 def launch_count():
     return _lib.load().b200md_launch_count()

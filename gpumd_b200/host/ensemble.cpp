@@ -280,3 +280,70 @@ void Ensemble_BAO_B200::compute2(
   op(1, time_step, group, atom);
   b2_find_thermo(*this, box.get_volume(), group, atom, thermo);
 }
+
+// ---- heat_lan / heat_nhc / heat_bdp: bath half, velocity-Verlet, bath half --------------------------
+Ensemble_HEAT_B200::Ensemble_HEAT_B200(
+  int t, int kind, int N, const std::vector<int>& group_sizes, const int* contents, int source, int sink,
+  double T, double Tc, double dT, double time_step, unsigned long long seed_source,
+  unsigned long long seed_sink)
+{
+  type = t;
+  temperature = T;
+  temperature_coupling = Tc;
+  set_move(*this, -1, nullptr);
+  if (b200md_heat_bath_create(
+        kind, N, (int)group_sizes.size(), group_sizes.data(), contents, source, sink, T, Tc, dT,
+        time_step, seed_source, seed_sink, &bath_) != B200MD_OK)
+    b2h_fail("Ensemble_HEAT_B200");
+}
+
+Ensemble_HEAT_B200::~Ensemble_HEAT_B200() { b200md_heat_bath_destroy(bath_); }
+
+void Ensemble_HEAT_B200::compute1(
+  const double time_step, const std::vector<Group>& group, Box&, Atom& atom, GPU_Vector<double>&)
+{
+  const int n = atom.number_of_atoms;
+  if (b200md_heat_bath_half(bath_, 0, n, n, atom.mass.data(), atom.velocity_per_atom.data(), nullptr) !=
+      B200MD_OK)
+    b2h_fail("Ensemble_HEAT_B200::compute1");
+  b2_velocity_verlet(*this, true, time_step, group, atom);
+}
+
+void Ensemble_HEAT_B200::compute2(
+  const double time_step, const std::vector<Group>& group, Box&, Atom& atom, GPU_Vector<double>&)
+{
+  b2_velocity_verlet(*this, false, time_step, group, atom);
+  const int n = atom.number_of_atoms;
+  if (b200md_heat_bath_half(bath_, 1, n, n, atom.mass.data(), atom.velocity_per_atom.data(), nullptr) !=
+      B200MD_OK)
+    b2h_fail("Ensemble_HEAT_B200::compute2");
+}
+
+void Ensemble_HEAT_B200::read_energy_transferred()
+{
+  if (b200md_heat_bath_energy(bath_, b2_energy_transferred, nullptr) != B200MD_OK)
+    b2h_fail("Ensemble_HEAT_B200::read_energy_transferred");
+}
+
+Ensemble_HEAT_LAN_B200::Ensemble_HEAT_LAN_B200(
+  int t, int mg, const double mv[3], int N, const std::vector<int>& group_sizes, const int* contents,
+  int source, int sink, double T, double Tc, double dT, unsigned long long seed_source,
+  unsigned long long seed_sink)
+    : Ensemble_HEAT_B200(t, 0, N, group_sizes, contents, source, sink, T, Tc, dT, 0.0, seed_source, seed_sink)
+{
+  set_move(*this, mg, mv);
+}
+
+Ensemble_HEAT_NHC_B200::Ensemble_HEAT_NHC_B200(
+  int t, int N, const std::vector<int>& group_sizes, const int* contents, int source, int sink, double T,
+  double Tc, double dT, double time_step)
+    : Ensemble_HEAT_B200(t, 1, N, group_sizes, contents, source, sink, T, Tc, dT, time_step, 0, 0)
+{
+}
+
+Ensemble_HEAT_BDP_B200::Ensemble_HEAT_BDP_B200(
+  int t, int N, const std::vector<int>& group_sizes, const int* contents, int source, int sink, double T,
+  double Tc, double dT, unsigned seed)
+    : Ensemble_HEAT_B200(t, 2, N, group_sizes, contents, source, sink, T, Tc, dT, 0.0, seed, 0)
+{
+}

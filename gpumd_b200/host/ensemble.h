@@ -162,3 +162,59 @@ private:
     GPU_Vector<double>& thermo);
   b200md_nhc* nhc_ = nullptr;
 };
+
+// Direct NEMD (heat_lan / heat_nhc / heat_bdp, types 22 / 21 / 23): a heat source at T + dT and a heat
+// sink at T - dT, groups `source` and `sink` of grouping method 0, whose sizes and Group::find_contents
+// list the caller passes (the reference reads them from group[0], integrate.cu:158-199).  The bath acts
+// before velocity-Verlet step 1 and after step 2 (heat_bdp: after step 2 only); like the reference,
+// compute2 does NOT call find_thermo, so thermo keeps its last value.  The energy transferred stays on
+// the device; read_energy_transferred() synchronises and fills energy_transferred[2].
+//   Ensemble_HEAT_LAN_B200 replaces Ensemble_LAN (heat), ensemble_lan.cu:43-85,128-269 (`move` allowed)
+//   Ensemble_HEAT_NHC_B200 replaces Ensemble_NHC (heat), ensemble_nhc.cu:52-91,239-326
+//   Ensemble_HEAT_BDP_B200 replaces Ensemble_BDP (heat), ensemble_bdp.cu:50-62,103-149
+class Ensemble_HEAT_B200 : public Ensemble, protected B200_Integrator
+{
+public:
+  ~Ensemble_HEAT_B200() override;
+  void compute1(
+    const double time_step, const std::vector<Group>& group, Box& box, Atom& atom,
+    GPU_Vector<double>& thermo) override;
+  void compute2(
+    const double time_step, const std::vector<Group>& group, Box& box, Atom& atom,
+    GPU_Vector<double>& thermo) override;
+  void read_energy_transferred();
+  double b2_energy_transferred[2] = {0.0, 0.0};
+
+protected:
+  Ensemble_HEAT_B200(
+    int t, int kind, int N, const std::vector<int>& group_sizes, const int* contents, int source,
+    int sink, double T, double Tc, double dT, double time_step, unsigned long long seed_source,
+    unsigned long long seed_sink);
+  b200md_heat_bath* bath_ = nullptr;
+};
+
+class Ensemble_HEAT_LAN_B200 : public Ensemble_HEAT_B200
+{
+public:
+  // seeds: the reference's next two rand() values (ensemble_lan.cu:78-81)
+  Ensemble_HEAT_LAN_B200(
+    int t, int mg, const double mv[3], int N, const std::vector<int>& group_sizes, const int* contents,
+    int source, int sink, double T, double Tc, double dT, unsigned long long seed_source,
+    unsigned long long seed_sink);
+};
+
+class Ensemble_HEAT_NHC_B200 : public Ensemble_HEAT_B200
+{
+public:
+  Ensemble_HEAT_NHC_B200(
+    int t, int N, const std::vector<int>& group_sizes, const int* contents, int source, int sink,
+    double T, double Tc, double dT, double time_step);
+};
+
+class Ensemble_HEAT_BDP_B200 : public Ensemble_HEAT_B200
+{
+public:
+  Ensemble_HEAT_BDP_B200(
+    int t, int N, const std::vector<int>& group_sizes, const int* contents, int source, int sink,
+    double T, double Tc, double dT, unsigned seed = 12345678u);
+};

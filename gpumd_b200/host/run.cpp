@@ -14,7 +14,7 @@
 // Keywords: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
 // nvt_ber|nvt_nhc|nvt_bdp T T tau, time_step <fs>, dump_thermo <n>, dump_xyz <n> <file> [precision
 // single|double] [mass velocity force potential virial], dump_restart <n>, compute_hac, compute_hnemd,
-// compute_shc, run <n>.  Anything else is an input error (exit 1), as in the reference.
+// compute_shc, ensemble heat_lan|heat_nhc|heat_bdp T Tc dT source sink, compute, run <n>.  Anything else is an input error (exit 1), as in the reference.
 #include "ensemble.h"
 #include "force.h"
 #include <algorithm>
@@ -331,8 +331,12 @@ private:
   // what the `ensemble` keyword asked for; the object itself is built at `run` from the time step
   // and atom count in force THEN, and rebuilt for every run (Integrate::initialize, integrate.cu:76-280)
   struct EnsembleSpec {
-    int type = -1; // 0 nve, 1 nvt_ber, 2 nvt_nhc, 3 nvt_lan, 4 nvt_bdp, 5 nvt_bao, 11 npt_ber
+    // 0 nve, 1 nvt_ber, 2 nvt_nhc, 3 nvt_lan, 4 nvt_bdp, 5 nvt_bao, 11 npt_ber, 21 heat_nhc, 22 heat_lan,
+    // 23 heat_bdp
+    int type = -1;
     double T = 0.0, Tc = 0.0;
+    double dT = 0.0;             // heat_*: the source is at T + dT, the sink at T - dT
+    int source = -1, sink = -1; // heat_*: group ids of grouping method 0
     // npt_ber: natural units, as integrate.cu:1150-1153 leaves them
     double target_p[6] = {0, 0, 0, 0, 0, 0}, p_coupling[6] = {0, 0, 0, 0, 0, 0};
     int num_p = 0;
@@ -373,6 +377,12 @@ private:
     int Nc = 0, direction = 0, num_omega = 0, group_method = -1, group_id = 0;
     double max_omega = 0.0;
   } shc_spec_;
+  // compute grouping_method sample_interval output_interval quantities... (compute.cu:595-660); reset
+  // after each run (Compute::postprocess, :69-88)
+  struct ComputeSpec {
+    int grouping_method = 0, sample_interval = 0, output_interval = 0; // sample_interval 0: off
+    unsigned mask = 0;
+  } compute_spec_;
   double global_time_ = 0.0; // natural units, as Run::global_time (run.cu:316)
   bool state_on_gpu_ = false;
   bool has_potential_ = false;
@@ -504,9 +514,12 @@ private:
           e.p_coupling[k] *= PRESSURE_UNIT_CONVERSION;
         }
         e.type = 11;
+      } else if (t[1] == "heat_nhc" || t[1] == "heat_lan" || t[1] == "heat_bdp") {
+        parse_heat(t, e);
       } else {
         input_error("supported by the b200md backend: ensemble nve | nvt_ber|nvt_nhc|nvt_bdp|nvt_lan|"
-                    "nvt_bao T T tau | npt_ber T T tau p.. C.. tau_p");
+                    "nvt_bao T T tau | npt_ber T T tau p.. C.. tau_p | heat_lan|heat_nhc|heat_bdp T Tc dT "
+                    "source sink");
       }
       ensemble_spec_ = e;
       if (e.type != 0)
@@ -556,6 +569,8 @@ private:
         input_error("compute_hac parameters should be positive integers.");
       printf("Compute HAC.\n    sample interval is %d.\n    Nc is %d\n    output_interval is %d\n",
              hac_spec_.interval, hac_spec_.Nc, hac_spec_.output_interval);
+    } else if (t[0] == "compute") {
+      parse_compute(t);
     } else if (t[0] == "compute_hnemd") {
       parse_compute_hnemd(t);
     } else if (t[0] == "compute_shc") {
@@ -579,6 +594,7 @@ private:
       hac_spec_ = HacSpec();
       hnemd_spec_ = HnemdSpec();
       shc_spec_ = ShcSpec();
+      compute_spec_ = ComputeSpec();
       force_.finalize();
       dump_thermo_ = 0; // non-propagating keywords are reset after each run (run.cu:329-340)
       dump_restart_ = 0;
@@ -586,6 +602,107 @@ private:
     } else {
       input_error("'" + t[0] + "' is not a keyword supported by the b200md backend.");
     }
+  }
+
+  // Integrate::parse_ensemble, heat branch (integrate.cu:479-493,716-768)
+  void parse_heat(const std::vector<std::string>& t, EnsembleSpec& e)
+  {
+    e.type = t[1] == "heat_nhc" ? 21 : (t[1] == "heat_lan" ? 22 : 23);
+    if (t.size() != 7)
+      input_error("ensemble " + t[1] + " should have 5 parameters.");
+    if (!valid_real(t[2], &e.T))
+      input_error("Temperature should be a number.");
+    if (e.T <= 0.0)
+      input_error("Temperature should > 0.");
+    if (!valid_real(t[3], &e.Tc))
+      input_error("Temperature coupling should be a number.");
+    if (e.Tc < 1.0)
+      input_error("Temperature coupling should >= 1.");
+    if (!valid_real(t[4], &e.dT))
+      input_error("Temperature difference should be a number.");
+    if (e.dT >= e.T || e.dT <= -e.T)
+      input_error("|Temperature difference| is too large.");
+    if (!valid_int(t[5], &e.source))
+      input_error("Group ID for heat source should be an integer.");
+    if (!valid_int(t[6], &e.sink))
+      input_error("Group ID for heat sink should be an integer.");
+    if (model_.group.size() < 1)
+      input_error("Cannot heat/cold without grouping method.");
+    if (e.source == e.sink)
+      input_error("Source and sink cannot be the same group.");
+    if (e.source < 0)
+      input_error("Group ID for heat source should >= 0.");
+    if (e.source >= model_.group[0].number)
+      input_error("Group ID for heat source should < #groups.");
+    if (e.sink < 0)
+      input_error("Group ID for heat sink should >= 0.");
+    if (e.sink >= model_.group[0].number)
+      input_error("Group ID for heat sink should < #groups.");
+    printf("Use %s heating/cooling: T = %g K, Tc = %g, dT = %g K, source %d, sink %d.\n", t[1].c_str(), e.T,
+           e.Tc, e.dT, e.source, e.sink);
+  }
+
+  // Compute::parse, compute.cu:595-660
+  void parse_compute(const std::vector<std::string>& t)
+  {
+    printf("Compute space and/or time average of:\n");
+    if (t.size() < 5)
+      input_error("compute should have at least 4 parameters.");
+    ComputeSpec c;
+    if (!valid_int(t[1], &c.grouping_method))
+      input_error("grouping method of compute should be integer.");
+    if (c.grouping_method < 0)
+      input_error("grouping method should >= 0.");
+    if (c.grouping_method >= (int)model_.group.size())
+      input_error("grouping method exceeds the bound.");
+    if (!valid_int(t[2], &c.sample_interval))
+      input_error("sampling interval of compute should be integer.");
+    if (c.sample_interval <= 0)
+      input_error("sampling interval of compute should > 0.");
+    if (!valid_int(t[3], &c.output_interval))
+      input_error("output interval of compute should be integer.");
+    if (c.output_interval <= 0)
+      input_error("output interval of compute should > 0.");
+    static const char* names[7] = {"temperature", "potential", "force", "virial", "jp", "jk", "momentum"};
+    for (size_t k = 4; k < t.size(); ++k) {
+      int q = 0;
+      while (q < 7 && t[k] != names[q])
+        ++q;
+      if (q == 7)
+        input_error("Invalid property for compute.");
+      c.mask |= 1u << q;
+      printf("    %s\n", names[q]);
+    }
+    printf("    using grouping method %d.\n", c.grouping_method);
+    printf("    with sampling interval %d.\n", c.sample_interval);
+    printf("    and output interval %d.\n", c.output_interval);
+    compute_spec_ = c;
+  }
+
+  // Compute::output_results, compute.cu:540-561: the averages, then (with temperature) the energy
+  // transferred to the source and sink baths.  A non-heat ensemble prints 0 for both (the reference
+  // prints its never-initialised energy_transferred there).
+  void write_compute(b200md_group_compute* cp, int num_values)
+  {
+    std::vector<double> v(num_values);
+    if (b200md_group_compute_take(cp, compute_spec_.output_interval, v.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute");
+    FILE* fc = fopen("compute.out", "a");
+    if (!fc)
+      input_error("Failed to open compute.out.");
+    for (double x : v)
+      fprintf(fc, "%15.6e", x);
+    if (compute_spec_.mask & B200MD_COMPUTE_TEMPERATURE) {
+      double e[2] = {0.0, 0.0};
+      if (auto* heat = dynamic_cast<Ensemble_HEAT_B200*>(ensemble_.get())) {
+        heat->read_energy_transferred();
+        e[0] = heat->b2_energy_transferred[0];
+        e[1] = heat->b2_energy_transferred[1];
+      }
+      fprintf(fc, "%15.6e%15.6e", e[0], e[1]);
+    }
+    fprintf(fc, "\n");
+    fclose(fc);
   }
 
   void parse_compute_hnemd(const std::vector<std::string>& t)
@@ -905,7 +1022,10 @@ private:
     // dump_thermo.cu:73-129: T, K, U, then sxx syy szz syz sxz sxy in GPa, then the box
     double th[8];
     thermo_.copy_to_host(th, 8);
-    const int N = model_.atom.number_of_atoms;
+    // the kinetic energy counts every atom but those of the fixed group (dump_thermo.cu:90-101)
+    int N = model_.atom.number_of_atoms;
+    if (fixed_group_ >= 0)
+      N -= model_.group[fixed_method_].cpu_size[fixed_group_];
     const double* h = model_.box.cpu_h;
     fprintf(fid, "%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e", th[0],
             1.5 * N * K_B * th[0], th[1], th[2] * PRESSURE_UNIT_CONVERSION,
@@ -930,7 +1050,7 @@ private:
           input_error("The fixed and moving groups must use the same grouping method.");
         if (move_group_ == fixed_group_)
           input_error("The fixed and moving groups cannot be the same.");
-        if (e.type != 1 && e.type != 2 && e.type != 4)
+        if (e.type != 1 && e.type != 2 && e.type != 4 && e.type != 22)
           input_error("It is only allowed to use nvt_ber, nvt_nhc, or nvt_bdp with a moving group.");
       }
       const int N = a.number_of_atoms;
@@ -951,6 +1071,24 @@ private:
         ensemble_.reset(new Ensemble_LAN_B200(3, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_lan.cu:39
       } else if (e.type == 5) {
         ensemble_.reset(new Ensemble_BAO_B200(5, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_bao.cu:39
+      } else if (e.type >= 21 && e.type <= 23) { // integrate.cu:158-199
+        const Group& g0 = model_.group[0];
+        if (e.type == 22) {
+          const unsigned long long seed_source = (unsigned long long)rand(); // ensemble_lan.cu:78-81
+          const unsigned long long seed_sink = (unsigned long long)rand();
+          ensemble_.reset(new Ensemble_HEAT_LAN_B200(22, move_group_, move_velocity_, N, g0.cpu_size,
+                                                     g0.contents.data(), e.source, e.sink, e.T, e.Tc, e.dT,
+                                                     seed_source, seed_sink));
+        } else if (e.type == 21) {
+          ensemble_.reset(new Ensemble_HEAT_NHC_B200(21, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
+                                                     e.T, e.Tc, e.dT, time_step_));
+        } else { // the B200MD_DEBUG_SEED rule of nvt_bdp (ensemble_bdp.cu:31-37)
+          const unsigned seed = std::getenv("B200MD_DEBUG_SEED")
+                                  ? 12345678u
+                                  : (unsigned)std::chrono::system_clock::now().time_since_epoch().count();
+          ensemble_.reset(new Ensemble_HEAT_BDP_B200(23, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
+                                                     e.T, e.Tc, e.dT, seed));
+        }
       } else if (e.type == 11) {
         const double no_rate[3] = {0, 0, 0};
         ensemble_.reset(new Ensemble_BER_B200(11, e.T, e.Tc, e.target_p, e.num_p, e.p_coupling, 0, 0, 0, no_rate));
@@ -1004,6 +1142,15 @@ private:
       if (rc != B200MD_OK)
         b2h_fail("compute_shc");
     }
+    b200md_group_compute* cp = nullptr;
+    int compute_values = 0;
+    if (compute_spec_.sample_interval > 0) { // Compute::preprocess, compute.cu:31-67
+      const Group& g = model_.group[compute_spec_.grouping_method];
+      if (b200md_group_compute_create(a.number_of_atoms, g.number, g.cpu_size.data(), g.contents.data(),
+                                      compute_spec_.mask, &cp) != B200MD_OK)
+        b2h_fail("compute");
+      compute_values = b200md_group_compute_columns(cp) * g.number;
+    }
     printf("Run %d steps.\n", number_of_steps);
     const auto t0 = std::chrono::high_resolution_clock::now();
     for (int step = 0; step < number_of_steps; ++step) {
@@ -1031,6 +1178,17 @@ private:
             fprintf(fk, "%25.15f", kappa[k]);
           fprintf(fk, "\n");
           fclose(fk);
+        }
+      }
+      if (cp && (step + 1) % compute_spec_.sample_interval == 0) { // Compute::process, compute.cu:351-538
+        if (b200md_group_compute_sample(cp, a.number_of_atoms, a.number_of_atoms, a.mass.data(),
+                                        a.potential_per_atom.data(), a.force_per_atom.data(),
+                                        a.virial_per_atom.data(), a.velocity_per_atom.data(),
+                                        nullptr) != B200MD_OK)
+          b2h_fail("compute");
+        if (((step + 1) / compute_spec_.sample_interval) % compute_spec_.output_interval == 0) {
+          force_.potentials[0]->check();
+          write_compute(cp, compute_values);
         }
       }
       if (shc && b200md_shc_sample(shc, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
@@ -1083,6 +1241,8 @@ private:
     }
     if (hnemd)
       b200md_hnemd_destroy(hnemd);
+    if (cp)
+      b200md_group_compute_destroy(cp);
     if (shc) {
       write_shc(shc, shc_groups);
       b200md_shc_destroy(shc);

@@ -90,6 +90,18 @@ SIGNATURES = {
     "b200md_shc_destroy": (None, [_vp]),
     "b200md_shc_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200md_shc_finish": (C.c_int, [_vp, C.c_double, C.c_int, C.c_double, _dp, _dp, _dp, _dp, _vp]),
+    "b200md_heat_bath_create": (C.c_int, [C.c_int, C.c_int, C.c_int, _ip, _ip, C.c_int, C.c_int, C.c_double,
+                                          C.c_double, C.c_double, C.c_double, C.c_ulonglong, C.c_ulonglong,
+                                          C.POINTER(_vp)]),
+    "b200md_heat_bath_destroy": (None, [_vp]),
+    "b200md_heat_bath_half": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "b200md_heat_bath_energy": (C.c_int, [_vp, _dp, _vp]),
+    "b200md_heat_bath_state": (C.c_int, [_vp, _dp, _vp]),
+    "b200md_group_compute_create": (C.c_int, [C.c_int, C.c_int, _ip, _ip, C.c_uint, C.POINTER(_vp)]),
+    "b200md_group_compute_destroy": (None, [_vp]),
+    "b200md_group_compute_columns": (C.c_int, [_vp]),
+    "b200md_group_compute_sample": (C.c_int, [_vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200md_group_compute_take": (C.c_int, [_vp, C.c_int, _dp, _vp]),
     "b200md_langevin_create": (C.c_int, [C.c_int, C.c_ulonglong, C.POINTER(_vp)]),
     "b200md_langevin_destroy": (None, [_vp]),
     "b200md_langevin_apply": (C.c_int, [_vp, C.c_int, C.c_int, C.c_double, C.c_double, _vp, _vp, _vp]),

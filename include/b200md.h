@@ -304,6 +304,68 @@ int b200md_shc_finish(
   b200md_shc* p, double time_step, int num_omega, double max_omega, double* ki, double* ko,
   double* shc_i, double* shc_o, void* stream);
 
+/* Direct NEMD: heat source / sink baths and group averages.
+ *   b200md_heat_bath_create  <- the heat branches of the Ensemble_LAN / _NHC / _BDP constructors
+ *                               (ensemble_lan.cu:43-85, ensemble_nhc.cu:52-91, ensemble_bdp.cu:50-62).
+ *                               kind 0 heat_lan (type 22), 1 heat_nhc (21), 2 heat_bdp (23).  Groups of
+ *                               grouping method 0: num_groups sizes and (host) contents in
+ *                               Group::find_contents order; source / sink are group ids.  The source
+ *                               bath is at T + dT, the sink at T - dT.  Tc = tau_T / time_step.
+ *                               heat_lan: cuRAND XORWOW states curand_init(seed_source, m, 0) for the m-th
+ *                               source atom and curand_init(seed_sink, m, 0) for the m-th sink atom (the
+ *                               reference passes its first and second rand(), ensemble_lan.cu:78-81);
+ *                               heat_bdp: ONE std::mt19937 stream seeded with (unsigned)seed_source
+ *                               (12345678 = the reference's -DDEBUG seed), source drawn before sink;
+ *                               heat_nhc: two chains with Q[0] scaled by 3 |group|; seeds unused.
+ *   b200md_heat_bath_half    <- integrate_heat_lan_half (ensemble_lan.cu:128-195; kick, no momentum
+ *                               correction), integrate_heat_nhc_1 / _2 (ensemble_nhc.cu:239-326) and
+ *                               integrate_heat_bdp_2 (ensemble_bdp.cu:103-149, after_vv2 only; a call with
+ *                               after_vv2 = 0 does nothing).  Call it before velocity-Verlet step 1
+ *                               (after_vv2 = 0) and after step 2 (after_vv2 = 1).  Asynchronous: the
+ *                               group sums, chains, generator and the energy transferred stay on the
+ *                               device.  No thermo is computed (the reference leaves it stale).
+ *   b200md_heat_bath_energy  <- Ensemble::energy_transferred[2] (eV, source then sink); synchronises
+ *   b200md_heat_bath_state   <- test hook, synchronises: out[44] = chain[2][12] (eta, v_eta, Q of the
+ *                               source / sink chains), stat[2][5] (sum m, sum m v_xyz, sum m v^2 per group
+ *                               before the last rescaling), vc[2][3], factor[2], energy[2]
+ *   b200md_group_compute_*   <- Compute (compute.cu:31-660).  what_mask: B200MD_COMPUTE_* bits; the
+ *                               columns come in the reference's fixed order (temperature, potential,
+ *                               force x3, virial x9 as xx xy xz yx yy yz zx zy zz, jp x3, jk x3,
+ *                               momentum x3), each a block of num_groups values.  _sample adds one sample
+ *                               (call it on the sampling steps only) into a device running sum with a
+ *                               fixed-order segmented reduction; _take (synchronises) writes the
+ *                               columns * num_groups averages over num_samples samples (temperature also
+ *                               divided by the group size, compute.cu:540-561) and resets the sum. */
+#define B200MD_COMPUTE_TEMPERATURE 1
+#define B200MD_COMPUTE_POTENTIAL 2
+#define B200MD_COMPUTE_FORCE 4
+#define B200MD_COMPUTE_VIRIAL 8
+#define B200MD_COMPUTE_JP 16
+#define B200MD_COMPUTE_JK 32
+#define B200MD_COMPUTE_MOMENTUM 64
+#define B200MD_COMPUTE_ALL 127
+typedef struct b200md_heat_bath b200md_heat_bath;
+int b200md_heat_bath_create(
+  int kind, int n, int num_groups, const int* group_sizes, const int* contents, int source, int sink,
+  double T, double Tc, double dT, double time_step, unsigned long long seed_source,
+  unsigned long long seed_sink, b200md_heat_bath** out);
+void b200md_heat_bath_destroy(b200md_heat_bath* p);
+int b200md_heat_bath_half(
+  b200md_heat_bath* p, int after_vv2, int n, int stride, const double* d_mass, double* d_velocity,
+  void* stream);
+int b200md_heat_bath_energy(b200md_heat_bath* p, double out2[2], void* stream);
+int b200md_heat_bath_state(b200md_heat_bath* p, double* out44, void* stream);
+typedef struct b200md_group_compute b200md_group_compute;
+int b200md_group_compute_create(
+  int n, int num_groups, const int* group_sizes, const int* contents, unsigned what_mask,
+  b200md_group_compute** out);
+void b200md_group_compute_destroy(b200md_group_compute* p);
+int b200md_group_compute_columns(const b200md_group_compute* p); /* -1 for a null handle */
+int b200md_group_compute_sample(
+  b200md_group_compute* p, int n, int stride, const double* d_mass, const double* d_potential,
+  const double* d_force, const double* d_virial, const double* d_velocity, void* stream);
+int b200md_group_compute_take(b200md_group_compute* p, int num_samples, double* out, void* stream);
+
 /* Langevin thermostats and the Berendsen barostat (SURVEY.md 8f rank 3):
  *   b200md_langevin_*         <- curand states + gpu_langevin + momentum correction,
  *                                src/integrate/langevin_utilities.cuh:26-127; one apply() = one

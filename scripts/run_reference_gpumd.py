@@ -29,6 +29,16 @@ BIN = ROOT / "oracle" / "_ref" / "gpumd_ref"
 OUT = ROOT / "refgpu_out"
 
 
+# the direct-NEMD cases; tests/test_gpu_nemd.py runs the same inputs through the b200md driver
+NEMD_GRAPHENE_RUN = ("ensemble nvt_ber 300 300 100\nfix 0\ntime_step 1\ndump_thermo 10\nrun 200\n"
+                     "ensemble heat_{kind} 300 100 10 1 8\nfix 0\ndump_thermo 100\n"
+                     "compute 0 10 10 temperature potential force virial jp jk momentum\n"
+                     "compute_shc 2 100 1 200 400.0 group 0 4\nrun 600\n")
+NEMD_PBTE_RUN = ("ensemble nvt_ber 300 300 100\ntime_step 1\ndump_thermo 10\nrun 100\n"
+                 "ensemble heat_lan 300 100 20 2 5\nfix 0\nmove 1 0 0.001 0\n"
+                 "compute 0 10 20 temperature jp jk\nrun 600\n")
+
+
 def write_model(path, s, symbols, vel=None):
     write_xyz(path, s, symbols, vel)
 
@@ -212,6 +222,20 @@ def main():
     d, i = run_case("hnemd_pbte", s, pbte_sym, GOLDEN / "nep_PbTe.txt",
                     "ensemble nvt_ber 300 300 100\ntime_step 1\ndump_thermo 10\ncompute_hnemd 10 0.00002 0 0\n"
                     "compute_shc 2 100 0 100 200 group 0 -1\nrun 250\n", vel)
+    infos.append(i)
+
+    # direct NEMD: the graphene sheet (FP64 Tersoff) with each heat bath after an nvt_ber run, and PbTe NEP
+    # with `fix`, `move` and heat_lan over six slabs along x.  Outputs: thermo.out, compute.out, shc.out
+    s = graphene_sheet()
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    for kind in ("lan", "nhc", "bdp"):
+        d, i = run_case(f"nemd_graphene_{kind}", s, ["C"], GOLDEN / "Graphene_Lindsay_2010_modified.txt",
+                        NEMD_GRAPHENE_RUN.format(kind=kind), vel)
+        infos.append(i)
+    s = rocksalt_pbte(12, rattle=0.02, seed=32)  # 13 824 atoms
+    s["group"] = np.minimum((s["pos"][0] / s["h"][0] * 6).astype(np.int32), 5)
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    d, i = run_case("nemd_pbte_lan", s, pbte_sym, GOLDEN / "nep_PbTe.txt", NEMD_PBTE_RUN, vel)
     infos.append(i)
 
     # ---- (3) throughput at the BASELINE sizes ----
