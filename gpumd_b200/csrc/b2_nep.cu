@@ -20,6 +20,11 @@ namespace {
 
 constexpr int BLK = 128;
 constexpr int MLP_BLK = 256;
+// k_angular_fused runs for models with a zero-padded descriptor of 32 (the width whose instances ptxas
+// compiles without spills at three blocks per SM; at 48 every instance spills) and where two of its
+// blocks fit an SM's 228 KB of shared memory (1 KB reserved per block)
+constexpr int FUSED_DIMP = 32;
+constexpr size_t FUSED_MAX_SMEM = 113 * 1024;
 
 __global__ void __launch_bounds__(BLK) k_split(B2NepView P, B2Box box)
 {
@@ -149,29 +154,8 @@ __global__ void __launch_bounds__(BLK) k_utable(B2NepView P)
   const int base = blockIdx.x * BLK;
   const int i = base + threadIdx.x;
   if (P.u_planes == 2) { // compact planes of the few-type kernels (b2_nep_radial.cuh)
-    if (i < P.n) {
-      constexpr int KQ = (K1 - 1) / 4;
-      const int t = P.atoms[i].type;
-      float4* U4 = reinterpret_cast<float4*>(P.U);
-      float* Uf = P.U + (size_t)P.nt * KQ * 4 * P.n;
-      for (int t2 = 0; t2 < P.nt; ++t2) {
-        const float* c = P.c_r + (size_t)(t * P.nt + t2) * P.nr1 * K1;
-        float u[K1];
-#pragma unroll
-        for (int k = 0; k < K1; ++k)
-          u[k] = 0.0f;
-        for (int n = 0; n < P.nr1; ++n) {
-          const float f = P.FpR[(size_t)n * P.n + i];
-#pragma unroll
-          for (int k = 0; k < K1; ++k)
-            u[k] = fmaf(f, __ldg(&c[n * K1 + k]), u[k]);
-        }
-#pragma unroll
-        for (int q = 0; q < KQ; ++q)
-          U4[(size_t)(t2 * KQ + q) * P.n + i] = make_float4(u[4 * q], u[4 * q + 1], u[4 * q + 2], u[4 * q + 3]);
-        Uf[(size_t)t2 * P.n + i] = u[K1 - 1];
-      }
-    }
+    if (i < P.n)
+      b2_utable_compact<K1>(P, i, P.atoms[i].type, [&](int n) { return P.FpR[(size_t)n * P.n + i]; });
     return;
   }
   if (P.u_planes) {
@@ -351,6 +335,8 @@ struct b200md_nep {
   int variant = 0;         // B200MD_NEP_VARIANT: kernel tuning variants for A/B measurements
   bool fuse_split = false; // many-type path: neighbour split inside the radial descriptor pass
   bool use_tc = false; // hidden layer on the tensor cores (k_mlp_tc) instead of k_mlp
+  bool ang_fused = false; // k_angular_fused instead of k_desc_angular2 + hidden layer + k_force_angular2
+  size_t fused_smem = 0;  // its dynamic shared memory per block
   bool slot_map = false;  // k_force_final2: thread per tile slot (type-pure warps); measured slower
                           // (H100, 1 M-atom PbTe: 1.26 vs 1.02 ms), B200MD_NEP_SLOTMAP=1 for A/B runs
   bool rad_direct = false; // many types: contract every pair on the spot (k_desc_radial<-1,...>), see nep_setup
@@ -594,6 +580,29 @@ int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool 
   return B200MD_OK;
 }
 
+template <int NT, int K1, int DIMP, bool ORTHO>
+int launch_fused_inst(const b200md_nep* p, const B2Box& box, cudaStream_t st)
+{
+  auto kern = k_angular_fused<NT, K1, DIMP, ORTHO>;
+  if (p->fused_smem > 48 * 1024)
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->fused_smem));
+  kern<<<grid_for(p->n, BLK), BLK, p->fused_smem, st>>>(
+    p->view, p->nb.plane0.p, p->nb.plane1.p, p->nb.planez.p, box, p->arev.p);
+  B2_LAUNCHED();
+  return B200MD_OK;
+}
+
+// the one hidden-layer width k_angular_fused is instantiated for (FUSED_DIMP, see nep_setup)
+template <int K1>
+int launch_angular_fused(const b200md_nep* p, const B2Box& box, cudaStream_t st)
+{
+  if (p->model.nt == 1)
+    return box.ortho ? launch_fused_inst<1, K1, FUSED_DIMP, true>(p, box, st)
+                     : launch_fused_inst<1, K1, FUSED_DIMP, false>(p, box, st);
+  return box.ortho ? launch_fused_inst<2, K1, FUSED_DIMP, true>(p, box, st)
+                   : launch_fused_inst<2, K1, FUSED_DIMP, false>(p, box, st);
+}
+
 template <int DIMP>
 int launch_mlp(const b200md_nep* p, cudaStream_t st)
 {
@@ -618,23 +627,17 @@ int launch_mlp(const b200md_nep* p, cudaStream_t st)
   } while (0)
 
 // stage ids reported by b200md_nep_profile_read / b200md_nep_stage_name
-enum { ST_NEIGHBOR, ST_DESC_R, ST_DESC_A, ST_MLP, ST_FORCE_A, ST_FORCE_FINAL, ST_COUNT };
+enum { ST_NEIGHBOR, ST_DESC_R, ST_DESC_A, ST_MLP, ST_FORCE_A, ST_FORCE_FINAL, ST_ANG_FUSED, ST_COUNT };
 const char* const STAGE_NAMES[ST_COUNT] = {
   "neighbor_update", "k_desc_radial", "k_desc_angular", "k_mlp", "k_force_angular",
-  "k_force_final"};
+  "k_force_final", "k_angular_fused"};
 
-int nep_pipeline(
-  b200md_nep* p, const B2Box& box, cudaStream_t st, double* d_pe, double* d_force, double* d_virial)
+// descriptor pass, hidden layer (+ U table) and angular force pass as separate kernels: models that do
+// not fit k_angular_fused, many types, and B200MD_NEP_MLP=simt / tc
+int angular_stages(b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
   const int n = p->n;
   StageProfiler& pf = p->prof;
-  pf.begin(st, ST_DESC_R);
-  switch (p->model.K1R) {
-    case 9: B2_TRY(dispatch_desc_radial<9>(p, box, st)); break;
-    case 13: B2_TRY(dispatch_desc_radial<13>(p, box, st)); break;
-    default: B2_TRY(dispatch_desc_radial<17>(p, box, st)); break;
-  }
-  pf.end(st, ST_DESC_R);
   pf.begin(st, ST_DESC_A);
   switch (p->model.K1A) {
     case 9: B2_TRY(launch_angular<9>(p, box, st, false)); break;
@@ -684,6 +687,31 @@ int nep_pipeline(
     default: B2_TRY(launch_angular<17>(p, box, st, true)); break;
   }
   pf.end(st, ST_FORCE_A);
+  return B200MD_OK;
+}
+
+int nep_pipeline(
+  b200md_nep* p, const B2Box& box, cudaStream_t st, double* d_pe, double* d_force, double* d_virial)
+{
+  StageProfiler& pf = p->prof;
+  pf.begin(st, ST_DESC_R);
+  switch (p->model.K1R) {
+    case 9: B2_TRY(dispatch_desc_radial<9>(p, box, st)); break;
+    case 13: B2_TRY(dispatch_desc_radial<13>(p, box, st)); break;
+    default: B2_TRY(dispatch_desc_radial<17>(p, box, st)); break;
+  }
+  pf.end(st, ST_DESC_R);
+  if (p->ang_fused) {
+    pf.begin(st, ST_ANG_FUSED);
+    switch (p->model.K1A) {
+      case 9: B2_TRY(launch_angular_fused<9>(p, box, st)); break;
+      case 13: B2_TRY(launch_angular_fused<13>(p, box, st)); break;
+      default: B2_TRY(launch_angular_fused<17>(p, box, st)); break;
+    }
+    pf.end(st, ST_ANG_FUSED);
+  } else {
+    B2_TRY(angular_stages(p, box, st));
+  }
   pf.begin(st, ST_FORCE_FINAL);
   switch (p->model.K1R) {
     case 9: B2_TRY(dispatch_force_final<9>(p, box, st, d_pe, d_force, d_virial)); break;
@@ -746,6 +774,18 @@ int nep_setup(b200md_nep* p, int num_atoms)
   if (const char* v = std::getenv("B200MD_NEP_CSTAGE"))
     p->ang_cstage = std::atoi(v) != 0;
   p->nb.tag_types = p->radial_v2; // skin entries carry the neighbour type (b2_nep_radial.cuh)
+  // Hidden layer and angular stages.  B200MD_NEP_MLP unset: k_angular_fused where the model fits its budget
+  // (FUSED_DIMP, FUSED_MAX_SMEM; DESIGN.md 3.2); then the SIMT layer is also the hidden layer of the
+  // generic kernels (B200MD_NEP_RADIAL=v1), which keeps the two paths bit-identical.  Otherwise the
+  // tensor cores unless the shapes do not fit them.  B200MD_NEP_MLP=simt / =tc select the SIMT / the
+  // tensor-core layer between separate angular kernels.
+  const char* mlp_env = std::getenv("B200MD_NEP_MLP");
+  const bool mlp_simt = mlp_env && std::strcmp(mlp_env, "simt") == 0;
+  p->fused_smem = b2_fused_smem_bytes(m.nt, m.na1, m.K1A, m.nneu, m.DIMP);
+  const bool fused_fits = m.nt <= 2 && !mlp_env && m.DIMP == FUSED_DIMP &&
+                          p->fused_smem <= FUSED_MAX_SMEM;
+  p->ang_fused = fused_fits && p->radial_v2;
+  p->use_tc = m.tc_ok && !mlp_simt && !fused_fits;
   if (p->radial_v2)
     B2_TRY(p->nb.enable_planes());
   const int pitch_r = (m.MN_radial + 7) / 8 * 8;
@@ -769,9 +809,11 @@ int nep_setup(b200md_nep* p, int num_atoms)
   B2_CUDA(p->nn_a.reserve(N));
   B2_CUDA(p->nl_a.reserve(N * m.MN_angular));
   B2_CUDA(p->q.reserve(N * m.dim));
-  B2_CUDA(p->sfx.reserve(N * m.na1 * B2_NABC));
-  B2_CUDA(p->FpR.reserve(N * m.nr1));
-  B2_CUDA(p->FpA.reserve(N * m.dim_angular));
+  if (!p->ang_fused) { // k_angular_fused keeps s and dU/dq on chip
+    B2_CUDA(p->sfx.reserve(N * m.na1 * B2_NABC));
+    B2_CUDA(p->FpR.reserve(N * m.nr1));
+    B2_CUDA(p->FpA.reserve(N * m.dim_angular));
+  }
   B2_CUDA(p->U.reserve(N * m.UST));
   B2_CUDA(p->f12.reserve(N * 3 * m.MN_angular));
   if (p->radial_v2)
@@ -848,9 +890,9 @@ int nep_setup(b200md_nep* p, int num_atoms)
   P.nn_a = p->nn_a.p;
   P.nl_a = p->nl_a.p;
   P.q = p->q.p;
-  P.sfx = p->sfx.p;
-  P.FpR = p->FpR.p;
-  P.FpA = p->FpA.p;
+  P.sfx = p->ang_fused ? nullptr : p->sfx.p;
+  P.FpR = p->ang_fused ? nullptr : p->FpR.p;
+  P.FpA = p->ang_fused ? nullptr : p->FpA.p;
   P.U = p->U.p;
   P.f12 = p->f12.p;
   P.acc = p->acc.p;
@@ -863,10 +905,6 @@ int nep_setup(b200md_nep* p, int num_atoms)
     P.skin_si = nv.skin_si;
     P.skin_sk = nv.skin_sk;
   }
-  // hidden layer: tensor cores unless the shapes do not fit or B200MD_NEP_MLP=simt asks for the
-  // SIMT kernel (kept for A/B measurements and for exotic layer sizes)
-  const char* mlp_env = std::getenv("B200MD_NEP_MLP");
-  p->use_tc = m.tc_ok && !(mlp_env && std::strcmp(mlp_env, "simt") == 0);
   if (p->use_tc) {
     int dev = 0;
     B2_CUDA(cudaGetDevice(&dev));

@@ -590,6 +590,74 @@ B2_HD void b2_harmonics_grad_dot(
   }
 }
 
+// Angular descriptor components of one radial channel from its sums s[abc]: the 3-body invariants
+// L = 1..4 (block L-1), then the 4-body (has222) and the 5-body (has1111) one; emit(block, value).
+// Component (block, n) sits at q[nr1 + block*na1 + n].
+template <class Emit>
+B2_HD void b2_ang_invariants(const float* s, int has222, int has1111, Emit emit)
+{
+  const float C3B[B2_NABC] = {B2_C3B_LIST};
+  int st = 0;
+#pragma unroll
+  for (int L = 1; L <= 4; ++L) {
+    float v = 0.0f;
+#pragma unroll
+    for (int k = 1; k < 2 * L + 1; ++k)
+      v = fmaf(C3B[st + k] * s[st + k], s[st + k], v);
+    v = 2.0f * v + C3B[st] * s[st] * s[st];
+    emit(L - 1, v);
+    st += 2 * L + 1;
+  }
+  int Lidx = 4;
+  if (has222) {
+    const float* t = &s[3];
+    const float v = B2_C4B0 * t[0] * t[0] * t[0] + B2_C4B1 * t[0] * (t[1] * t[1] + t[2] * t[2]) +
+                    B2_C4B2 * t[0] * (t[3] * t[3] + t[4] * t[4]) +
+                    B2_C4B3 * t[3] * (t[2] * t[2] - t[1] * t[1]) + B2_C4B4 * t[1] * t[2] * t[4];
+    emit(Lidx, v);
+    ++Lidx;
+  }
+  if (has1111) {
+    const float s0 = s[0] * s[0], tt = s[1] * s[1] + s[2] * s[2];
+    emit(Lidx, B2_C5B0 * s0 * s0 + B2_C5B1 * s0 * tt + B2_C5B2 * tt * tt);
+  }
+}
+
+// dU/ds[abc] of one radial channel: 3-body weights plus the chain-rule terms of the 4- and 5-body
+// invariants.  F[L-1] = dU/dq of the L-th 3-body component, F[4] of the 4-body, F[5] of the 5-body one
+// (ignored when the model lacks them).
+B2_HD void b2_ang_weights(const float* s, const float* F6, int has222, int has1111, float* wv)
+{
+  const float C3B[B2_NABC] = {B2_C3B_LIST};
+  int st = 0;
+#pragma unroll
+  for (int L = 1; L <= 4; ++L) {
+    const float F = F6[L - 1];
+    wv[st] = 2.0f * F * C3B[st] * s[st];
+#pragma unroll
+    for (int k = 1; k < 2 * L + 1; ++k)
+      wv[st + k] = 4.0f * F * C3B[st + k] * s[st + k];
+    st += 2 * L + 1;
+  }
+  if (has222) {
+    const float F = F6[4];
+    const float* t = &s[3];
+    wv[3] += F * (3.0f * B2_C4B0 * t[0] * t[0] + B2_C4B1 * (t[1] * t[1] + t[2] * t[2]) +
+                  B2_C4B2 * (t[3] * t[3] + t[4] * t[4]));
+    wv[4] += F * (2.0f * B2_C4B1 * t[0] * t[1] - 2.0f * B2_C4B3 * t[3] * t[1] + B2_C4B4 * t[2] * t[4]);
+    wv[5] += F * (2.0f * B2_C4B1 * t[0] * t[2] + 2.0f * B2_C4B3 * t[3] * t[2] + B2_C4B4 * t[1] * t[4]);
+    wv[6] += F * (2.0f * B2_C4B2 * t[0] * t[3] + B2_C4B3 * (t[2] * t[2] - t[1] * t[1]));
+    wv[7] += F * (2.0f * B2_C4B2 * t[0] * t[4] + B2_C4B4 * t[1] * t[2]);
+  }
+  if (has1111) {
+    const float F = F6[5];
+    const float tt = s[1] * s[1] + s[2] * s[2];
+    wv[0] += F * (4.0f * B2_C5B0 * s[0] * s[0] * s[0] + 2.0f * B2_C5B1 * tt * s[0]);
+    wv[1] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[1] + 4.0f * B2_C5B2 * tt * s[1]);
+    wv[2] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[2] + 4.0f * B2_C5B2 * tt * s[2]);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // angular descriptor (angular half of find_descriptor, nep.cu:549-581, find_q
 // nep_utilities.cuh:1819-1872).  Processes the radial index n in chunks of NCH so that the
@@ -694,24 +762,19 @@ B2_HD void b2_body_desc_angular(
 // per-atom MLP (apply_ann_one_layer[_nep5], nep_utilities.cuh:169-194, 285-310; nep.cu:583-657)
 // plus the radial pre-contraction U_i[t][k] = sum_n Fp_i[n] c[t_i,t,n,k].
 // ---------------------------------------------------------------------------------------------
-// w0_all / b0_all / w1_all: [nt][nneu][DIMP], [nt][nneu], [nt][nneu] -- either the global tables
-// (GLOBAL_W = true, read through the read-only path) or a shared-memory copy staged by the block.
+// The per-atom core: scaled descriptor q[DIMP] (zero-padded) in, site energy out, dU/dq (already
+// multiplied by q_scaler) in Fp[DIMP].  w0 / b0 / w1 are the rows of the atom's type.  Shared by
+// b2_body_mlp and k_angular_fused (b2_nep_angular.cuh), so both produce the same bits.
 template <int DIMP, bool GLOBAL_W>
-B2_HD void b2_body_mlp(
-  int i, const B2NepView& P, const float* w0_all, const float* b0_all, const float* w1_all)
+B2_HD float b2_mlp_core(
+  const float* q, const float4* w0, const float* b0, const float* w1, int nneu, float bias,
+  const float* q_scaler, float* Fp)
 {
-  const int t = P.atoms[i].type;
-  float q[DIMP], Fp[DIMP];
 #pragma unroll
-  for (int d = 0; d < DIMP; ++d) {
-    q[d] = (d < P.dim) ? P.q[(size_t)d * P.n + i] * B2_LDG(&P.q_scaler[d]) : 0.0f;
+  for (int d = 0; d < DIMP; ++d)
     Fp[d] = 0.0f;
-  }
-  const float4* w0 = reinterpret_cast<const float4*>(w0_all + (size_t)t * P.nneu * DIMP);
-  const float* b0 = b0_all + (size_t)t * P.nneu;
-  const float* w1 = w1_all + (size_t)t * P.nneu;
   float F = 0.0f;
-  for (int n = 0; n < P.nneu; ++n) {
+  for (int n = 0; n < nneu; ++n) {
     const float4* row = w0 + (size_t)n * (DIMP / 4);
     float4 w[DIMP / 4];
 #pragma unroll
@@ -737,11 +800,28 @@ B2_HD void b2_body_mlp(
       Fp[4 * d + 3] = fmaf(coef, w[d].w, Fp[4 * d + 3]);
     }
   }
-  F -= B2_LDG(&P.bias[t]);
-  P.acc[i] = (double)F;
+  F -= bias;
 #pragma unroll
   for (int d = 0; d < DIMP; ++d)
-    Fp[d] *= B2_LDG(&P.q_scaler[d]);
+    Fp[d] *= B2_LDG(&q_scaler[d]);
+  return F;
+}
+
+// w0_all / b0_all / w1_all: [nt][nneu][DIMP], [nt][nneu], [nt][nneu] -- either the global tables
+// (GLOBAL_W = true, read through the read-only path) or a shared-memory copy staged by the block.
+template <int DIMP, bool GLOBAL_W>
+B2_HD void b2_body_mlp(
+  int i, const B2NepView& P, const float* w0_all, const float* b0_all, const float* w1_all)
+{
+  const int t = P.atoms[i].type;
+  float q[DIMP], Fp[DIMP];
+#pragma unroll
+  for (int d = 0; d < DIMP; ++d)
+    q[d] = (d < P.dim) ? P.q[(size_t)d * P.n + i] * B2_LDG(&P.q_scaler[d]) : 0.0f;
+  const float F = b2_mlp_core<DIMP, GLOBAL_W>(
+    q, reinterpret_cast<const float4*>(w0_all + (size_t)t * P.nneu * DIMP), b0_all + (size_t)t * P.nneu,
+    w1_all + (size_t)t * P.nneu, P.nneu, B2_LDG(&P.bias[t]), P.q_scaler, Fp);
+  P.acc[i] = (double)F;
   // dU/dq: radial part first (input of the U-table contraction), then the angular part
 #pragma unroll
   for (int d = 0; d < DIMP; ++d) {
@@ -775,6 +855,40 @@ B2_HD void b2_body_utable(int i, const B2NepView& P)
 #pragma unroll
     for (int k = 0; k < KP; ++k)
       U[t2 * KP + k] = u[k];
+  }
+}
+
+// same contraction into the compact planes of the few-type kernels (B2NepView::u_planes == 2):
+// KQ = (K1-1)/4 float4 planes U4[(t2*KQ + q)*n + i] and a float plane [t2*n + i] for k = K1-1.
+// fr(n) = dU/dq[n] of atom i (type t), n < nr1.  Shared by k_utable and k_angular_fused.
+template <int K1, class FpR>
+B2_HD void b2_utable_compact(const B2NepView& P, int i, int t, FpR fr)
+{
+  constexpr int KQ = (K1 - 1) / 4;
+  float4* U4 = reinterpret_cast<float4*>(P.U);
+  float* Uf = P.U + (size_t)P.nt * KQ * 4 * P.n;
+  for (int t2 = 0; t2 < P.nt; ++t2) {
+    const float* c = P.c_r + (size_t)(t * P.nt + t2) * P.nr1 * K1;
+    float u[K1];
+#pragma unroll
+    for (int k = 0; k < K1; ++k)
+      u[k] = 0.0f;
+    for (int n = 0; n < P.nr1; ++n) {
+      const float f = fr(n);
+#pragma unroll
+      for (int k = 0; k < K1; ++k)
+        u[k] = fmaf(f, B2_LDG(&c[n * K1 + k]), u[k]);
+    }
+#pragma unroll
+    for (int q = 0; q < KQ; ++q) {
+      float4 v;
+      v.x = u[4 * q];
+      v.y = u[4 * q + 1];
+      v.z = u[4 * q + 2];
+      v.w = u[4 * q + 3];
+      U4[(size_t)(t2 * KQ + q) * P.n + i] = v;
+    }
+    Uf[(size_t)t2 * P.n + i] = u[K1 - 1];
   }
 }
 

@@ -1,4 +1,4 @@
-// b2_nep_angular.cuh -- the two angular kernels of the NEP path for models with one or two atom types
+// b2_nep_angular.cuh -- the angular kernels of the NEP path for models with one or two atom types
 // (device only), on the layout of b2_nep_radial.cuh.  Same arithmetic per pair, op for op, as
 // b2_body_desc_angular / b2_body_force_angular in b2_nep.cuh (which tests/emu runs on the host and
 // which stay the many-type path); what differs is everything around the arithmetic:
@@ -14,7 +14,11 @@
 //     read as float4s (the per-pair W / Wp contraction needs a quarter of the shared-memory loads);
 //   * the force kernel also finds, for each pair (i, j), the slot of i in j's angular list and stores
 //     it (arev), so that the pair reduction in k_force_final2 (b2_reduce_angular_planes) gathers f21
-//     directly instead of walking a binary search of dependent loads.
+//     directly instead of walking a binary search of dependent loads;
+//   * k_angular_fused runs the descriptor, the hidden layer, the U table and the partial forces of one
+//     atom in one thread, so s, dU/dq and the weights never leave the SM (the default where the model
+//     fits it, see nep_setup); the two-kernel pair with k_mlp / k_mlp_tc in between stays for the models
+//     that do not fit and for B200MD_NEP_MLP=simt / tc.  All of them call the same bodies below.
 #pragma once
 #include "b2_nep_radial.cuh"
 
@@ -46,30 +50,24 @@ __device__ __forceinline__ void b2_stage_ctab(const B2NepView& P, float4* dst, i
 }
 
 // ---------------------------------------------------------------------------------------------
-// Angular descriptor.  The radial index n is processed in chunks of NCH channels so that the NCH*24
-// accumulators stay in registers; each chunk walks the (short) angular list once.  NCH = 3 at three
-// blocks per SM (146 registers for PbTe, no spills) measured faster on an H100 (400 W, 1 M-atom PbTe:
-// 0.41 ms) than one pass with NCH = 5 at two blocks per SM (198 registers, 0.48 ms); NCH = 5 at three
-// blocks spills.
+// Angular descriptor of sorted atom i (record a1).  The radial index n is processed in chunks of NCH
+// channels so that the NCH*24 accumulators stay in registers; each chunk walks the (short) angular
+// list once.  NCH = 3 at three blocks per SM (146 registers for PbTe, no spills) measured faster on an
+// H100 (400 W, 1 M-atom PbTe: 0.41 ms) than one pass with NCH = 5 at two blocks per SM (198 registers,
+// 0.48 ms); NCH = 5 at three blocks spills.
+// emit_q(k, v): descriptor component k (nr1 <= k < dim); emit_s(g, v): float4 group g = n*6 + abc/4 of
+// the sums s[n][abc].
 // ---------------------------------------------------------------------------------------------
-template <int NT, int K1, int NCH, bool ORTHO>
-__global__ void __launch_bounds__(128, 3) k_desc_angular2(
-  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
-  const double* __restrict__ pz, const B2Box box)
+template <int NT, int K1, int NCH, bool ORTHO, class EmitQ, class EmitS>
+__device__ __forceinline__ void b2_ang_desc_atom(
+  const B2NepView& P, const int4* __restrict__ p0, const double* __restrict__ pz, const B2Box& box,
+  int i, const B2Rec& a1, const float4* ctab_s, EmitQ emit_q, EmitS emit_s)
 {
   static_assert(NT == 1 || NT == 2, "few-type path");
   constexpr int KQ = (K1 + 3) / 4;
-  extern __shared__ float4 ctab_s[];
-  b2_stage_ctab(P, ctab_s, KQ);
-  __syncthreads();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P.n)
-    return;
-  const float C3B[B2_NABC] = {B2_C3B_LIST};
   const B2GeoR geo = b2_geo_pinned(box);
   const unsigned N = (unsigned)P.n;
   const int na1 = P.na1;
-  const B2Rec a1 = b2_rec_load(p0, p1, i);
   const int t1 = a1.t;
   float rcv[NT], rciv[NT];
   b2_ang_cutoffs<NT>(P, t1, rcv, rciv);
@@ -79,17 +77,6 @@ __global__ void __launch_bounds__(128, 3) k_desc_angular2(
     crow[t] = ctab_s + (t1 * P.nt + (t < P.nt ? t : 0)) * na1 * KQ;
   const int* __restrict__ list = P.nl_a;
   const int nn = P.nn_a[i];
-  // descriptor component k of this atom: tile-major copy (k_mlp_tc) or SoA columns
-  float* const qb = P.qt ? P.qt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.q + i;
-  // With the tile-major copy the angular components are collected in shared memory (qs[(k-nr1)*128 + tid],
-  // after the coefficient table) and written once at the end as 16-byte groups: written where they are
-  // formed, one 4-byte store per component, the groups of a tile row would reach HBM as partial sectors
-  // in two passes over the list.
-  float* const qs = reinterpret_cast<float*>(ctab_s + P.nt * P.nt * na1 * KQ) + threadIdx.x;
-  auto qat = [&](int k) -> float* {
-    return P.qt ? qs + (size_t)(k - P.nr1) * 128 : qb + (size_t)k * N;
-  };
-  float4* __restrict__ sf4 = reinterpret_cast<float4*>(P.sfx);
   for (int n0 = 0; n0 < na1; n0 += NCH) {
     float s[NCH][B2_NABC];
 #pragma unroll
@@ -140,38 +127,42 @@ __global__ void __launch_bounds__(128, 3) k_desc_angular2(
     for (int c = 0; c < NCH; ++c) {
       const int n = n0 + c;
       if (n < na1) {
-        // 3-body invariants, L = 1..4: q[nr1 + (L-1)*na1 + n]
-        int st = 0;
-#pragma unroll
-        for (int L = 1; L <= 4; ++L) {
-          float v = 0.0f;
-#pragma unroll
-          for (int k = 1; k < 2 * L + 1; ++k)
-            v = fmaf(C3B[st + k] * s[c][st + k], s[c][st + k], v);
-          v = 2.0f * v + C3B[st] * s[c][st] * s[c][st];
-          *qat(P.nr1 + (L - 1) * na1 + n) = v;
-          st += 2 * L + 1;
-        }
-        int Lidx = 4;
-        if (P.has222) {
-          const float* t = &s[c][3];
-          const float v = B2_C4B0 * t[0] * t[0] * t[0] + B2_C4B1 * t[0] * (t[1] * t[1] + t[2] * t[2]) +
-                          B2_C4B2 * t[0] * (t[3] * t[3] + t[4] * t[4]) +
-                          B2_C4B3 * t[3] * (t[2] * t[2] - t[1] * t[1]) + B2_C4B4 * t[1] * t[2] * t[4];
-          *qat(P.nr1 + Lidx * na1 + n) = v;
-          ++Lidx;
-        }
-        if (P.has1111) {
-          const float s0 = s[c][0] * s[c][0], tt = s[c][1] * s[c][1] + s[c][2] * s[c][2];
-          *qat(P.nr1 + Lidx * na1 + n) = B2_C5B0 * s0 * s0 + B2_C5B1 * s0 * tt + B2_C5B2 * tt * tt;
-        }
+        b2_ang_invariants(s[c], P.has222, P.has1111,
+                          [&](int blk, float v) { emit_q(P.nr1 + blk * na1 + n, v); });
 #pragma unroll
         for (int g = 0; g < B2_ABC4; ++g)
-          sf4[(size_t)(n * B2_ABC4 + g) * N + i] =
-            make_float4(s[c][4 * g], s[c][4 * g + 1], s[c][4 * g + 2], s[c][4 * g + 3]);
+          emit_s(n * B2_ABC4 + g, make_float4(s[c][4 * g], s[c][4 * g + 1], s[c][4 * g + 2], s[c][4 * g + 3]));
       }
     }
   }
+}
+
+template <int NT, int K1, int NCH, bool ORTHO>
+__global__ void __launch_bounds__(128, 3) k_desc_angular2(
+  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
+  const double* __restrict__ pz, const B2Box box)
+{
+  constexpr int KQ = (K1 + 3) / 4;
+  extern __shared__ float4 ctab_s[];
+  b2_stage_ctab(P, ctab_s, KQ);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const unsigned N = (unsigned)P.n;
+  const B2Rec a1 = b2_rec_load(p0, p1, i);
+  // descriptor component k of this atom: tile-major copy (k_mlp_tc) or SoA columns
+  float* const qb = P.qt ? P.qt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.q + i;
+  // With the tile-major copy the angular components are collected in shared memory (qs[(k-nr1)*128 + tid],
+  // after the coefficient table) and written once at the end as 16-byte groups: written where they are
+  // formed, one 4-byte store per component, the groups of a tile row would reach HBM as partial sectors
+  // in two passes over the list.
+  float* const qs = reinterpret_cast<float*>(ctab_s + P.nt * P.nt * P.na1 * KQ) + threadIdx.x;
+  float4* __restrict__ sf4 = reinterpret_cast<float4*>(P.sfx);
+  b2_ang_desc_atom<NT, K1, NCH, ORTHO>(
+    P, p0, pz, box, i, a1, ctab_s,
+    [&](int k, float v) { *(P.qt ? qs + (size_t)(k - P.nr1) * 128 : qb + (size_t)k * N) = v; },
+    [&](int g, float4 v) { sf4[(size_t)g * N + i] = v; });
   if (P.qt) {
     const int klo = P.nr1, khi = P.dim;
     for (int k0 = klo & ~3; k0 < khi; k0 += 4) {
@@ -195,108 +186,17 @@ __global__ void __launch_bounds__(128, 3) k_desc_angular2(
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ constexpr int b2_ang_ws4(int na1) { return B2_ABC4 * na1 + 1; }
 
+// The pair loop of sorted atom i (record a1): w = its row of weights dU/ds[n][abc] (float4 group
+// n*6 + abc/4), ctab_s the staged coefficient table.
 template <int NT, int K1, bool ORTHO>
-__global__ void __launch_bounds__(128, 3) k_force_angular2(
-  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
-  const double* __restrict__ pz, const B2Box box, int* __restrict__ arev)
+__device__ __forceinline__ void b2_ang_force_pairs(
+  const B2NepView& P, const int4* __restrict__ p0, const double* __restrict__ pz, const B2Box& box,
+  int i, const B2Rec& a1, const float4* w, const float4* ctab_s, int* __restrict__ arev)
 {
-  static_assert(NT == 1 || NT == 2, "few-type path");
   constexpr int KQ = (K1 + 3) / 4;
-  extern __shared__ float4 fa_smem[];
-  const int na1 = P.na1;
-  const int WS4 = b2_ang_ws4(na1);
-  float4* const ctab_s = fa_smem + blockDim.x * WS4;
-  b2_stage_ctab(P, ctab_s, KQ);
-  __syncthreads();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P.n)
-    return;
-  const float C3B[B2_NABC] = {B2_C3B_LIST};
   const unsigned N = (unsigned)P.n;
-  float4* const w = fa_smem + threadIdx.x * WS4;
-  // dU/dq of this atom: tile-major copy written by k_mlp_tc (component d at fbase + (d/4)*512 + d%4),
-  // or the SoA columns FpA[(d - nr1)*N + i] of the SIMT layer
-  const float* fbase = P.fpt ? P.fpt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.FpA + i;
-  auto FpAt = [&](int da) -> float { // da = index inside the angular part
-    if (P.fpt) {
-      const int d = P.nr1 + da;
-      return fbase[(size_t)(d >> 2) * 512 + (d & 3)];
-    }
-    return fbase[(size_t)da * N];
-  };
-  // ---- weights (as b2_body_force_angular) ----
-  const float4* __restrict__ sf4 = reinterpret_cast<const float4*>(P.sfx);
-  // the sums and dU/dq of NB channels are fetched together before any of them is used, so a warp waits
-  // for one memory latency per NB channels instead of one per channel (H100, 400 W, 1 M-atom PbTe:
-  // 0.42 ms with NB = 3 against 0.44 with NB = 1 and NB = 5; NB = 5 needs 168 registers and spills)
-  constexpr int NB = 3;
-  for (int n0 = 0; n0 < na1; n0 += NB) {
-    float4 sv[NB][B2_ABC4];
-    float Fv[NB][6];
-#pragma unroll
-    for (int c = 0; c < NB; ++c) {
-      const int n = n0 + c;
-      if (n < na1) {
-#pragma unroll
-        for (int g = 0; g < B2_ABC4; ++g)
-          sv[c][g] = sf4[(size_t)(n * B2_ABC4 + g) * N + i];
-#pragma unroll
-        for (int L = 0; L < 4; ++L)
-          Fv[c][L] = FpAt(L * na1 + n);
-        Fv[c][4] = P.has222 ? FpAt(4 * na1 + n) : 0.0f;
-        Fv[c][5] = P.has1111 ? FpAt((4 + (P.has222 ? 1 : 0)) * na1 + n) : 0.0f;
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < NB; ++c) {
-    const int n = n0 + c;
-    if (n >= na1)
-      break;
-    float s[B2_NABC];
-#pragma unroll
-    for (int g = 0; g < B2_ABC4; ++g) {
-      const float4 v = sv[c][g];
-      s[4 * g] = v.x;
-      s[4 * g + 1] = v.y;
-      s[4 * g + 2] = v.z;
-      s[4 * g + 3] = v.w;
-    }
-    float wv[B2_NABC];
-    int st = 0;
-#pragma unroll
-    for (int L = 1; L <= 4; ++L) {
-      const float F = Fv[c][L - 1];
-      wv[st] = 2.0f * F * C3B[st] * s[st];
-#pragma unroll
-      for (int k = 1; k < 2 * L + 1; ++k)
-        wv[st + k] = 4.0f * F * C3B[st + k] * s[st + k];
-      st += 2 * L + 1;
-    }
-    if (P.has222) {
-      const float F = Fv[c][4];
-      const float* t = &s[3];
-      wv[3] += F * (3.0f * B2_C4B0 * t[0] * t[0] + B2_C4B1 * (t[1] * t[1] + t[2] * t[2]) +
-                    B2_C4B2 * (t[3] * t[3] + t[4] * t[4]));
-      wv[4] += F * (2.0f * B2_C4B1 * t[0] * t[1] - 2.0f * B2_C4B3 * t[3] * t[1] + B2_C4B4 * t[2] * t[4]);
-      wv[5] += F * (2.0f * B2_C4B1 * t[0] * t[2] + 2.0f * B2_C4B3 * t[3] * t[2] + B2_C4B4 * t[1] * t[4]);
-      wv[6] += F * (2.0f * B2_C4B2 * t[0] * t[3] + B2_C4B3 * (t[2] * t[2] - t[1] * t[1]));
-      wv[7] += F * (2.0f * B2_C4B2 * t[0] * t[4] + B2_C4B4 * t[1] * t[2]);
-    }
-    if (P.has1111) {
-      const float F = Fv[c][5];
-      const float tt = s[1] * s[1] + s[2] * s[2];
-      wv[0] += F * (4.0f * B2_C5B0 * s[0] * s[0] * s[0] + 2.0f * B2_C5B1 * tt * s[0]);
-      wv[1] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[1] + 4.0f * B2_C5B2 * tt * s[1]);
-      wv[2] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[2] + 4.0f * B2_C5B2 * tt * s[2]);
-    }
-#pragma unroll
-    for (int g = 0; g < B2_ABC4; ++g)
-      w[n * B2_ABC4 + g] = make_float4(wv[4 * g], wv[4 * g + 1], wv[4 * g + 2], wv[4 * g + 3]);
-    }
-  }
-  // ---- pairs ----
+  const int na1 = P.na1;
   const B2GeoR geo = b2_geo_pinned(box);
-  const B2Rec a1 = b2_rec_load(p0, p1, i);
   const int t1 = a1.t;
   float rcv[NT], rciv[NT];
   b2_ang_cutoffs<NT>(P, t1, rcv, rciv);
@@ -405,6 +305,198 @@ __global__ void __launch_bounds__(128, 3) k_force_angular2(
     P.f12[2 * plane + slot] = fmaf(rad, zh, gz * dinv);
     arev[slot] = hit ? below : 0;
   }
+}
+
+template <int NT, int K1, bool ORTHO>
+__global__ void __launch_bounds__(128, 3) k_force_angular2(
+  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
+  const double* __restrict__ pz, const B2Box box, int* __restrict__ arev)
+{
+  static_assert(NT == 1 || NT == 2, "few-type path");
+  constexpr int KQ = (K1 + 3) / 4;
+  extern __shared__ float4 fa_smem[];
+  const int na1 = P.na1;
+  const int WS4 = b2_ang_ws4(na1);
+  float4* const ctab_s = fa_smem + blockDim.x * WS4;
+  b2_stage_ctab(P, ctab_s, KQ);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const unsigned N = (unsigned)P.n;
+  float4* const w = fa_smem + threadIdx.x * WS4;
+  // dU/dq of this atom: tile-major copy written by k_mlp_tc (component d at fbase + (d/4)*512 + d%4),
+  // or the SoA columns FpA[(d - nr1)*N + i] of the SIMT layer
+  const float* fbase = P.fpt ? P.fpt + b2_tile_offset(P.DKT, P.tile_slot[i], 0) : P.FpA + i;
+  auto FpAt = [&](int da) -> float { // da = index inside the angular part
+    if (P.fpt) {
+      const int d = P.nr1 + da;
+      return fbase[(size_t)(d >> 2) * 512 + (d & 3)];
+    }
+    return fbase[(size_t)da * N];
+  };
+  // ---- weights ----
+  const float4* __restrict__ sf4 = reinterpret_cast<const float4*>(P.sfx);
+  // the sums and dU/dq of NB channels are fetched together before any of them is used, so a warp waits
+  // for one memory latency per NB channels instead of one per channel (H100, 400 W, 1 M-atom PbTe:
+  // 0.42 ms with NB = 3 against 0.44 with NB = 1 and NB = 5; NB = 5 needs 168 registers and spills)
+  constexpr int NB = 3;
+  for (int n0 = 0; n0 < na1; n0 += NB) {
+    float4 sv[NB][B2_ABC4];
+    float Fv[NB][6];
+#pragma unroll
+    for (int c = 0; c < NB; ++c) {
+      const int n = n0 + c;
+      if (n < na1) {
+#pragma unroll
+        for (int g = 0; g < B2_ABC4; ++g)
+          sv[c][g] = sf4[(size_t)(n * B2_ABC4 + g) * N + i];
+#pragma unroll
+        for (int L = 0; L < 4; ++L)
+          Fv[c][L] = FpAt(L * na1 + n);
+        Fv[c][4] = P.has222 ? FpAt(4 * na1 + n) : 0.0f;
+        Fv[c][5] = P.has1111 ? FpAt((4 + (P.has222 ? 1 : 0)) * na1 + n) : 0.0f;
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < NB; ++c) {
+      const int n = n0 + c;
+      if (n >= na1)
+        break;
+      float s[B2_NABC];
+#pragma unroll
+      for (int g = 0; g < B2_ABC4; ++g) {
+        const float4 v = sv[c][g];
+        s[4 * g] = v.x;
+        s[4 * g + 1] = v.y;
+        s[4 * g + 2] = v.z;
+        s[4 * g + 3] = v.w;
+      }
+      float wv[B2_NABC];
+      b2_ang_weights(s, Fv[c], P.has222, P.has1111, wv);
+#pragma unroll
+      for (int g = 0; g < B2_ABC4; ++g)
+        w[n * B2_ABC4 + g] = make_float4(wv[4 * g], wv[4 * g + 1], wv[4 * g + 2], wv[4 * g + 3]);
+    }
+  }
+  // ---- pairs ----
+  b2_ang_force_pairs<NT, K1, ORTHO>(P, p0, pz, box, i, b2_rec_load(p0, p1, i), w, ctab_s, arev);
+}
+
+// ---------------------------------------------------------------------------------------------
+// k_angular_fused: descriptor, hidden layer, U table and angular partial forces of one sorted atom in
+// one thread, for models that fit its budget (b2_fused_smem_bytes, DIMP = 32; nep_setup).  Nothing in
+// the chain depends on another atom's result, so s[n][abc], dU/dq and dU/ds stay on the SM:
+//   1. descriptor (b2_ang_desc_atom): s goes to the thread's shared-memory row, the angular components
+//      of q to the SoA columns P.q (they stay observable, b200md_nep_export_descriptors; the thread
+//      reads them back at once, from L2);
+//   2. hidden layer (b2_mlp_core) from the radial part of q that k_desc_radial2 wrote and the angular
+//      part, weights from a shared-memory copy; site energy to acc[i];
+//   3. U table rows (b2_utable_compact) from the radial part of dU/dq;
+//   4. weights dU/ds (b2_ang_weights) in place over s;
+//   5. pair loop (b2_ang_force_pairs): f12 and arev.
+// Every step calls the body the five-kernel path calls, so the results are bit-identical to it with the
+// SIMT hidden layer.  dU/dq is copied to a thread-local array because steps 3 and 4 index it at run time
+// (nr1, na1 are model values); that array lives in local memory, which L1 / L2 cache.
+// Dynamic shared memory: 128 rows of b2_ang_ws4(na1) float4s, the coefficient table, then w0 of each
+// type at a stride of b2_fused_w0_stride4 float4s (odd: a warp holding both types reads the two rows
+// on distinct banks), b0 and w1.
+// ---------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int b2_fused_w0_stride4(int nneu, int dimp) { return (nneu * dimp / 4) | 1; }
+
+__host__ __device__ constexpr size_t b2_fused_smem_bytes(int nt, int na1, int k1a, int nneu, int dimp)
+{
+  return (size_t)128 * b2_ang_ws4(na1) * 16 + (size_t)nt * nt * na1 * ((k1a + 3) / 4) * 16 +
+         (size_t)nt * b2_fused_w0_stride4(nneu, dimp) * 16 + (size_t)2 * nt * nneu * 4;
+}
+
+template <int NT, int K1, int DIMP, bool ORTHO>
+__global__ void __launch_bounds__(128, 3) k_angular_fused(
+  const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
+  const double* __restrict__ pz, const B2Box box, int* __restrict__ arev)
+{
+  static_assert(NT == 1 || NT == 2, "few-type path");
+  constexpr int KQ = (K1 + 3) / 4;
+  extern __shared__ float4 af_smem[];
+  const int na1 = P.na1, nneu = P.nneu;
+  const int WS4 = b2_ang_ws4(na1);
+  float4* const ctab_s = af_smem + blockDim.x * WS4;
+  float4* const w0_s = ctab_s + P.nt * P.nt * na1 * KQ;
+  const int wst4 = b2_fused_w0_stride4(nneu, DIMP);
+  float* const b0_s = reinterpret_cast<float*>(w0_s + P.nt * wst4);
+  float* const w1_s = b0_s + P.nt * nneu;
+  b2_stage_ctab(P, ctab_s, KQ);
+  {
+    const int row4 = nneu * DIMP / 4;
+    const float4* src = reinterpret_cast<const float4*>(P.w0p);
+    for (int e = threadIdx.x; e < P.nt * row4; e += blockDim.x) {
+      const int t = e / row4;
+      w0_s[t * wst4 + (e - t * row4)] = __ldg(&src[e]);
+    }
+    for (int e = threadIdx.x; e < P.nt * nneu; e += blockDim.x) {
+      b0_s[e] = __ldg(&P.b0[e]);
+      w1_s[e] = __ldg(&P.w1[e]);
+    }
+  }
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const unsigned N = (unsigned)P.n;
+  float4* const row = af_smem + threadIdx.x * WS4;
+  const B2Rec a1 = b2_rec_load(p0, p1, i);
+  // 1. descriptor
+  b2_ang_desc_atom<NT, K1, 3, ORTHO>(
+    P, p0, pz, box, i, a1, ctab_s, [&](int k, float v) { P.q[(size_t)k * N + i] = v; },
+    [&](int g, float4 v) { row[g] = v; });
+  // 2. hidden layer
+  const int t = a1.t;
+  float fl[DIMP]; // dU/dq, indexed at run time below
+  {
+    float q[DIMP], Fp[DIMP];
+#pragma unroll
+    for (int d = 0; d < DIMP; ++d)
+      q[d] = (d < P.dim) ? P.q[(size_t)d * N + i] * __ldg(&P.q_scaler[d]) : 0.0f;
+    const float F = b2_mlp_core<DIMP, false>(q, w0_s + t * wst4, b0_s + t * nneu, w1_s + t * nneu, nneu,
+                                             __ldg(&P.bias[t]), P.q_scaler, Fp);
+    P.acc[i] = (double)F;
+#pragma unroll
+    for (int d = 0; d < DIMP; ++d)
+      fl[d] = Fp[d];
+  }
+  // 3. U table
+  auto fr = [&](int n) { return fl[n]; };
+  switch (P.K1R) {
+    case 9: b2_utable_compact<9>(P, i, t, fr); break;
+    case 13: b2_utable_compact<13>(P, i, t, fr); break;
+    default: b2_utable_compact<17>(P, i, t, fr); break;
+  }
+  // 4. weights over s
+  const float* fa = fl + P.nr1;
+  for (int n = 0; n < na1; ++n) {
+    float s[B2_NABC];
+#pragma unroll
+    for (int g = 0; g < B2_ABC4; ++g) {
+      const float4 v = row[n * B2_ABC4 + g];
+      s[4 * g] = v.x;
+      s[4 * g + 1] = v.y;
+      s[4 * g + 2] = v.z;
+      s[4 * g + 3] = v.w;
+    }
+    float F6[6];
+#pragma unroll
+    for (int L = 0; L < 4; ++L)
+      F6[L] = fa[L * na1 + n];
+    F6[4] = P.has222 ? fa[4 * na1 + n] : 0.0f;
+    F6[5] = P.has1111 ? fa[(4 + (P.has222 ? 1 : 0)) * na1 + n] : 0.0f;
+    float wv[B2_NABC];
+    b2_ang_weights(s, F6, P.has222, P.has1111, wv);
+#pragma unroll
+    for (int g = 0; g < B2_ABC4; ++g)
+      row[n * B2_ABC4 + g] = make_float4(wv[4 * g], wv[4 * g + 1], wv[4 * g + 2], wv[4 * g + 3]);
+  }
+  // 5. pairs
+  b2_ang_force_pairs<NT, K1, ORTHO>(P, p0, pz, box, i, a1, row, ctab_s, arev);
 }
 
 } // namespace b2
