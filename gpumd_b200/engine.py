@@ -475,6 +475,123 @@ class SHC:
         return ki.reshape(g, nk), ko.reshape(g, nk), si[:g * nw].reshape(g, nw), so[:g * nw].reshape(g, nw)
 
 
+def _groups_arg(num_atoms, groups):
+    """(sizes, contents) of b200md_*_create: None -> the whole system in atom order."""
+    if groups is None:
+        return np.array([int(num_atoms)], np.int32), None
+    sizes = np.array([len(g) for g in groups], np.int32)
+    contents = np.ascontiguousarray(np.concatenate([np.asarray(g, np.int32) for g in groups]))
+    return sizes, contents
+
+
+class _Correlation:
+    """The shared shape of DOS, SDC and MSD: process(step, atom) every step, postprocess() at the end
+    (or, for MSD, at any time).  groups: None for the whole system of num_atoms atoms, or a list of int
+    arrays, the atom indices of each output group (Group::find_contents order)."""
+    _kind = ""
+
+    def _create(self, head, num_atoms, groups, tail=()):
+        _require_cuda()
+        self._L = _lib.load()
+        sizes, contents = _groups_arg(num_atoms, groups)
+        self.num_groups = sizes.shape[0]
+        ip = C.POINTER(C.c_int)
+        h = C.c_void_p()
+        _lib.check(getattr(self._L, f"b200md_{self._kind}_create")(
+            *head, self.num_groups, sizes.ctypes.data_as(ip),
+            None if contents is None else contents.ctypes.data_as(ip), *tail, C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            getattr(self._L, f"b200md_{self._kind}_destroy")(self._h)
+            self._h = None
+
+    def _sample(self, step, n, x):
+        _lib.check(getattr(self._L, f"b200md_{self._kind}_sample")(self._h, int(step), n, n, _ptr(x), _stream()))
+
+    def _finish(self, rows_a, rows_b):
+        a, b = np.zeros(self.num_groups * 3 * rows_a), np.zeros(self.num_groups * 3 * rows_b)
+        dp = C.POINTER(C.c_double)
+        _lib.check(getattr(self._L, f"b200md_{self._kind}_finish")(
+            self._h, a.ctypes.data_as(dp), b.ctypes.data_as(dp), _stream()))
+        return a.reshape(self.num_groups, 3, rows_a), b.reshape(self.num_groups, 3, rows_b)
+
+
+class DOS(_Correlation):
+    """compute_dos, src/measure/dos.cu.  The masses are gathered from atom.mass once, here.
+    postprocess() returns mvac [num_groups, 3, Nc] (normalised) and dos [num_groups, 3, num_dos_points]."""
+    _kind = "dos"
+
+    def __init__(self, sample_interval, Nc, omega_max, number_of_steps, time_step, atom, groups=None,
+                 num_dos_points=None):
+        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
+        self.num_dos_points = self.Nc if num_dos_points is None else int(num_dos_points)
+        n = atom.number_of_atoms
+        self._create((self.Nc, self.sample_interval, int(number_of_steps), float(time_step), float(omega_max),
+                      self.num_dos_points), n, groups, (n, _ptr(atom.mass)))
+
+    def process(self, step, atom):
+        self._sample(step, atom.number_of_atoms, atom.velocity_per_atom)
+
+    def postprocess(self):
+        return self._finish(self.Nc, self.num_dos_points)
+
+
+class SDC(_Correlation):
+    """compute_sdc, src/measure/sdc.cu.  postprocess() returns vac (A^2/ps^2) and sdc (A^2/ps), each
+    [num_groups, 3, Nc]."""
+    _kind = "sdc"
+
+    def __init__(self, sample_interval, Nc, number_of_steps, time_step, num_atoms=None, groups=None):
+        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
+        self._create((self.Nc, self.sample_interval, int(number_of_steps), float(time_step)), num_atoms, groups)
+
+    def process(self, step, atom):
+        self._sample(step, atom.number_of_atoms, atom.velocity_per_atom)
+
+    def postprocess(self):
+        return self._finish(self.Nc, self.Nc)
+
+
+class MSD(_Correlation):
+    """compute_msd, src/measure/msd.cu, on the unwrapped positions of an UnwrappedPosition.
+    postprocess() returns msd (A^2) and sdc (A^2/ps), each [num_groups, 3, Nc]; it may be called during
+    the run and then covers every time origin sampled so far."""
+    _kind = "msd"
+
+    def __init__(self, sample_interval, Nc, number_of_steps, time_step, num_atoms=None, groups=None):
+        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
+        self._create((self.Nc, self.sample_interval, int(number_of_steps), float(time_step)), num_atoms, groups)
+
+    def process(self, step, unwrapped):
+        """unwrapped: an UnwrappedPosition (or a [3 * n] float64 device tensor)."""
+        x = getattr(unwrapped, "unwrapped_position", unwrapped)
+        self._sample(step, x.shape[0] // 3, x)
+
+    def postprocess(self):
+        return self._finish(self.Nc, self.Nc)
+
+
+class UnwrappedPosition:
+    """atom.unwrapped_position of the reference (msd.cu:471-477, integrate.cu:347-374): starts as a copy
+    of the current positions; call begin(atom) before an ensemble's compute1 and end(atom) after it."""
+
+    def __init__(self, atom):
+        _require_cuda()
+        self._L = _lib.load()
+        self.unwrapped_position = atom.position_per_atom.clone()
+        self.position_temp = torch.empty_like(atom.position_per_atom)
+
+    def begin(self, atom):
+        _lib.check(self._L.b200md_unwrap_begin(atom.number_of_atoms, _ptr(atom.position_per_atom),
+                                               _ptr(self.position_temp), _stream()))
+
+    def end(self, atom):
+        _lib.check(self._L.b200md_unwrap_end(atom.number_of_atoms, _ptr(atom.position_per_atom),
+                                             _ptr(self.position_temp), _ptr(self.unwrapped_position), _stream()))
+
+
 class Ensemble_NVE:
     """NVE integrator, src/integrate/ensemble_nve.cu:31-95 (velocity-Verlet + thermo)."""
 

@@ -14,7 +14,8 @@
 // Keywords: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
 // nvt_ber|nvt_nhc|nvt_bdp T T tau, time_step <fs>, dump_thermo <n>, dump_xyz <n> <file> [precision
 // single|double] [mass velocity force potential virial], dump_restart <n>, compute_hac, compute_hnemd,
-// compute_shc, ensemble heat_lan|heat_nhc|heat_bdp T Tc dT source sink, compute, run <n>.  Anything else is an input error (exit 1), as in the reference.
+// compute_shc, ensemble heat_lan|heat_nhc|heat_bdp T Tc dT source sink, compute, compute_dos,
+// compute_sdc, compute_msd, run <n>.  Anything else is an input error (exit 1), as in the reference.
 #include "ensemble.h"
 #include "force.h"
 #include <algorithm>
@@ -383,6 +384,18 @@ private:
     int grouping_method = 0, sample_interval = 0, output_interval = 0; // sample_interval 0: off
     unsigned mask = 0;
   } compute_spec_;
+  // compute_dos / compute_sdc / compute_msd (dos.cu:153-202, sdc.cu:300-338, msd.cu:481-541); reset after
+  // each run (the postprocess of each).  sample_interval 0: off; group_method -1: the whole system
+  struct CorrSpec {
+    int sample_interval = 0, Nc = 0, group_method = -1, group_id = -1;
+    double omega_max = 0.0; // DOS
+    int num_dos_points = -1; // DOS; -1: Nc
+    bool all_groups = false; // MSD
+    int save_every = -1;     // MSD
+  } dos_spec_, sdc_spec_, msd_spec_;
+  // atom.unwrapped_position of the reference: tracked from the first run with compute_msd on, in every
+  // later run too (msd.cu:471-477, integrate.cu:347-374)
+  GPU_Vector<double> unwrapped_, position_old_;
   double global_time_ = 0.0; // natural units, as Run::global_time (run.cu:316)
   bool state_on_gpu_ = false;
   bool has_potential_ = false;
@@ -575,6 +588,12 @@ private:
       parse_compute_hnemd(t);
     } else if (t[0] == "compute_shc") {
       parse_compute_shc(t);
+    } else if (t[0] == "compute_dos") {
+      parse_compute_dos(t);
+    } else if (t[0] == "compute_sdc") {
+      parse_compute_sdc(t);
+    } else if (t[0] == "compute_msd") {
+      parse_compute_msd(t);
     } else if (t[0] == "dump_restart") {
       if (t.size() != 2 || std::atoi(t[1].c_str()) <= 0)
         input_error("dump_restart should have 1 positive parameter (the interval).");
@@ -595,6 +614,7 @@ private:
       hnemd_spec_ = HnemdSpec();
       shc_spec_ = ShcSpec();
       compute_spec_ = ComputeSpec();
+      dos_spec_ = sdc_spec_ = msd_spec_ = CorrSpec();
       force_.finalize();
       dump_thermo_ = 0; // non-propagating keywords are reset after each run (run.cu:329-340)
       dump_restart_ = 0;
@@ -818,6 +838,251 @@ private:
       for (int nw = 0; nw < c.num_omega; ++nw) // shc_i, shc_o in A eV = A eV/ps/THz
         fprintf(fid, "%g %g %g\n", (nw + 1) * d_omega, si[(size_t)g * c.num_omega + nw],
                 so[(size_t)g * c.num_omega + nw]);
+    }
+    fclose(fid);
+  }
+
+  // the sample interval and Nc that all three correlation keywords start with
+  void parse_interval_nc(const std::vector<std::string>& t, CorrSpec& c)
+  {
+    if (!valid_int(t[1], &c.sample_interval))
+      input_error("sample interval should be an integer.");
+    if (c.sample_interval <= 0)
+      input_error("sample interval should be positive.");
+    printf("    sample interval is %d.\n", c.sample_interval);
+    if (!valid_int(t[2], &c.Nc))
+      input_error("number of correlation steps should be an integer.");
+    if (c.Nc <= 0)
+      input_error("number of correlation steps should be positive.");
+    printf("    number of correlation steps is %d.\n", c.Nc);
+  }
+
+  // parse_group, src/measure/parse_utilities.cu:27-62
+  void parse_group(const std::vector<std::string>& t, bool allow_all_groups, size_t& k, CorrSpec& c)
+  {
+    if (k + 3 > t.size())
+      input_error("Not enough arguments for option 'group'.");
+    if (!valid_int(t[k + 1], &c.group_method))
+      input_error("Grouping method should be an integer.");
+    if (c.group_method < 0)
+      input_error("Grouping method should >= 0.");
+    if (c.group_method >= (int)model_.group.size())
+      input_error("Grouping method should < number of grouping methods.");
+    if (!valid_int(t[k + 2], &c.group_id))
+      input_error("Group ID should be an integer.");
+    if (c.group_id >= model_.group[c.group_method].number)
+      input_error("Group ID should < number of groups.");
+    if (c.group_id < 0 && !allow_all_groups)
+      input_error("group ID should >= 0.");
+    printf("    grouping method is %d and group ID is %d.\n", c.group_method, c.group_id);
+    k += 2;
+  }
+
+  // DOS::parse, dos.cu:153-202
+  void parse_compute_dos(const std::vector<std::string>& t)
+  {
+    printf("Compute phonon DOS.\n");
+    if (t.size() < 4)
+      input_error("compute_dos should have at least 3 parameters.");
+    if (t.size() > 9)
+      input_error("compute_dos has too many parameters.");
+    CorrSpec c;
+    parse_interval_nc(t, c);
+    if (!valid_real(t[3], &c.omega_max))
+      input_error("maximal angular frequency should be a number.");
+    if (c.omega_max <= 0)
+      input_error("maximal angular frequency should be positive.");
+    printf("    maximal angular frequency is %g THz.\n", c.omega_max);
+    for (size_t k = 4; k < t.size(); k++) {
+      if (t[k] == "group") {
+        parse_group(t, true, k, c);
+      } else if (t[k] == "num_dos_points") {
+        if (k + 2 > t.size())
+          input_error("Not enough arguments for option 'num_dos_points'.");
+        if (!valid_int(t[k + 1], &c.num_dos_points))
+          input_error("number of DOS points should be an integer.");
+        if (c.num_dos_points < 1)
+          input_error("number of DOS points must be > 0.");
+        k += 1;
+        printf("    num_dos_points is %d.\n", c.num_dos_points);
+      } else {
+        input_error("Unrecognized argument in compute_dos.");
+      }
+    }
+    dos_spec_ = c;
+  }
+
+  // SDC::parse, sdc.cu:300-338
+  void parse_compute_sdc(const std::vector<std::string>& t)
+  {
+    printf("Compute self diffusion coefficient (SDC).\n");
+    if (t.size() < 3)
+      input_error("compute_sdc should have at least 2 parameters.");
+    if (t.size() > 6)
+      input_error("compute_sdc has too many parameters.");
+    CorrSpec c;
+    parse_interval_nc(t, c);
+    for (size_t k = 3; k < t.size(); k++) {
+      if (t[k] == "group")
+        parse_group(t, false, k, c);
+      else
+        input_error("Unrecognized argument in compute_sdc.");
+    }
+    sdc_spec_ = c;
+  }
+
+  // MSD::parse, msd.cu:481-541.  all_groups reads the method after the keyword (the reference reads
+  // param[4], which is that position in the documented form `compute_msd <i> <Nc> all_groups <m>`)
+  void parse_compute_msd(const std::vector<std::string>& t)
+  {
+    printf("Compute mean square displacement (MSD).\n");
+    if (t.size() < 3)
+      input_error("compute_msd should have at least 2 parameters.");
+    if (t.size() > 8)
+      input_error("compute_msd has too many parameters.");
+    CorrSpec c;
+    parse_interval_nc(t, c);
+    for (size_t k = 3; k < t.size(); k++) {
+      if (t[k] == "group") {
+        parse_group(t, false, k, c);
+      } else if (t[k] == "all_groups") {
+        c.all_groups = true;
+        if (k + 2 > t.size() || !valid_int(t[k + 1], &c.group_method))
+          input_error("Grouping method should be an integer.");
+        if (c.group_method < 0)
+          input_error("Grouping method should >= 0.");
+        if (c.group_method >= (int)model_.group.size())
+          input_error("Grouping method should < number of grouping methods.");
+        printf("    will compute MSD for all groups in grouping %d.\n", c.group_method);
+        k += 1;
+      } else if (t[k] == "save_every") {
+        if (k + 2 > t.size() || !valid_int(t[k + 1], &c.save_every))
+          input_error("save_every should be an integer.");
+        printf("    will save a copy of the MSD every %d steps.\n", c.save_every);
+        k += 1;
+      } else {
+        input_error("Unrecognized argument in compute_msd.");
+      }
+    }
+    if (c.all_groups && c.group_method >= 0 && c.group_id >= 0)
+      input_error("Cannot compute MSD over a single group and all groups at the same time");
+    msd_spec_ = c;
+  }
+
+  // the output groups of a correlation keyword as (sizes, contents): the whole system, one group, or
+  // every group of the method (`group m -1` for DOS, `all_groups m` for MSD)
+  const int* corr_groups(const CorrSpec& c, std::vector<int>& sizes) const
+  {
+    sizes.assign(1, model_.atom.number_of_atoms);
+    if (c.group_method < 0)
+      return nullptr; // the whole system in atom order
+    const Group& g = model_.group[c.group_method];
+    if (c.all_groups || c.group_id < 0) {
+      sizes = g.cpu_size;
+      return g.contents.data();
+    }
+    sizes.assign(1, g.cpu_size[c.group_id]);
+    return g.contents.data() + g.cpu_size_sum[c.group_id];
+  }
+
+  // DOS::output_vac / output_dos, dos.cu:429-448,483-503: appended, no header, group after group
+  void write_dos(b200md_dos* dos, int num_groups)
+  {
+    const CorrSpec& c = dos_spec_;
+    const int Nc = c.Nc, nw = c.num_dos_points;
+    std::vector<double> mvac((size_t)num_groups * 3 * Nc), d((size_t)num_groups * 3 * nw);
+    if (b200md_dos_finish(dos, mvac.data(), d.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute_dos");
+    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
+    FILE* fid = fopen("mvac.out", "a");
+    if (!fid)
+      input_error("Failed to open mvac.out.");
+    for (int g = 0; g < num_groups; ++g) {
+      const double* v = mvac.data() + (size_t)g * 3 * Nc;
+      for (int nc = 0; nc < Nc; nc++)
+        fprintf(fid, "%g %g %g %g\n", nc * dt_in_ps, v[nc], v[Nc + nc], v[2 * Nc + nc]);
+    }
+    fclose(fid);
+    const double d_omega = c.omega_max / nw;
+    fid = fopen("dos.out", "a");
+    if (!fid)
+      input_error("Failed to open dos.out.");
+    for (int g = 0; g < num_groups; ++g) {
+      const double* v = d.data() + (size_t)g * 3 * nw;
+      for (int k = 0; k < nw; k++)
+        fprintf(fid, "%g %g %g %g\n", d_omega + d_omega * k, v[k], v[nw + k], v[2 * nw + k]);
+    }
+    fclose(fid);
+  }
+
+  // SDC::postprocess, sdc.cu:259-285 (the cell at the end of the run)
+  void write_sdc(b200md_sdc* sdc, int num_atoms)
+  {
+    const CorrSpec& c = sdc_spec_;
+    const int Nc = c.Nc;
+    std::vector<double> vac((size_t)3 * Nc), s((size_t)3 * Nc);
+    if (b200md_sdc_finish(sdc, vac.data(), s.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute_sdc");
+    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
+    FILE* fid = fopen("sdc.out", "a");
+    if (!fid)
+      input_error("Failed to open sdc.out.");
+    fprintf(fid, "# compute_sdc %d %d", c.sample_interval, Nc);
+    if (c.group_method >= 0)
+      fprintf(fid, " group %d %d", c.group_method, c.group_id);
+    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n", num_atoms);
+    const double* h = model_.box.cpu_h;
+    fprintf(fid, "# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6], h[1], h[4],
+            h[7], h[2], h[5], h[8]);
+    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
+    fprintf(fid, "# columns time_ps vacx vacy vacz sdcx sdcy sdcz\n");
+    for (int nc = 0; nc < Nc; nc++)
+      fprintf(fid, "%g %g %g %g %g %g %g\n", nc * dt_in_ps, vac[nc], vac[Nc + nc], vac[2 * Nc + nc], s[nc],
+              s[Nc + nc], s[2 * Nc + nc]);
+    fclose(fid);
+  }
+
+  // MSD::write, msd.cu:365-449; h: the cell at the start of the run (msd.cu:254-255)
+  void write_msd(b200md_msd* msd, const char* filename, const std::vector<int>& sizes, int num_atoms,
+                 const double* h)
+  {
+    const CorrSpec& c = msd_spec_;
+    const int Nc = c.Nc, ng = (int)sizes.size();
+    std::vector<double> m((size_t)ng * 3 * Nc), s(m.size());
+    if (b200md_msd_finish(msd, m.data(), s.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute_msd");
+    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
+    FILE* fid = fopen(filename, "a");
+    if (!fid)
+      input_error(std::string("Failed to open ") + filename + ".");
+    fprintf(fid, "# compute_msd %d %d", c.sample_interval, Nc);
+    if (c.all_groups)
+      fprintf(fid, " all_groups %d", c.group_method);
+    else if (c.group_method >= 0)
+      fprintf(fid, " group %d %d", c.group_method, c.group_id);
+    if (c.save_every > 0)
+      fprintf(fid, " save_every %d", c.save_every);
+    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n# num_groups %d\n# num_atoms_per_group", num_atoms, ng);
+    for (int g = 0; g < ng; ++g)
+      fprintf(fid, " %d", sizes[g]);
+    fprintf(fid, "\n# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6], h[1], h[4],
+            h[7], h[2], h[5], h[8]);
+    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
+    fprintf(fid, "# columns time_ps");
+    if (!c.all_groups)
+      fprintf(fid, " msdx msdy msdz sdcx sdcy sdcz");
+    else
+      for (int g = 0; g < ng; ++g)
+        fprintf(fid, " msdx_%d msdy_%d msdz_%d sdcx_%d sdcy_%d sdcz_%d", g, g, g, g, g, g);
+    fprintf(fid, "\n");
+    for (int nc = 0; nc < Nc; nc++) {
+      fprintf(fid, "%g", nc * dt_in_ps);
+      for (int g = 0; g < ng; g++) {
+        const double* a = m.data() + (size_t)g * 3 * Nc;
+        const double* b = s.data() + (size_t)g * 3 * Nc;
+        fprintf(fid, "% g %g %g %g %g %g", a[nc], a[Nc + nc], a[2 * Nc + nc], b[nc], b[Nc + nc], b[2 * Nc + nc]);
+      }
+      fprintf(fid, "\n");
     }
     fclose(fid);
   }
@@ -1151,10 +1416,64 @@ private:
         b2h_fail("compute");
       compute_values = b200md_group_compute_columns(cp) * g.number;
     }
+    // DOS::preprocess, SDC::preprocess, MSD::preprocess (dos.cu:204-218, sdc.cu:132-155, msd.cu:205-267)
+    const int N = a.number_of_atoms;
+    b200md_dos* dos = nullptr;
+    std::vector<int> dos_sizes, sdc_sizes, msd_sizes;
+    if (dos_spec_.sample_interval > 0) {
+      CorrSpec& c = dos_spec_;
+      if (c.num_dos_points < 0)
+        c.num_dos_points = c.Nc;
+      const int* contents = corr_groups(c, dos_sizes);
+      const int rc = b200md_dos_create(c.Nc, c.sample_interval, number_of_steps, time_step_, c.omega_max,
+                                       c.num_dos_points, (int)dos_sizes.size(), dos_sizes.data(), contents, N,
+                                       a.mass.data(), &dos);
+      if (rc == B200MD_ERR_ARG)
+        input_error(std::string("compute_dos: ") + b200md_last_error());
+      if (rc != B200MD_OK)
+        b2h_fail("compute_dos");
+    }
+    b200md_sdc* sdc = nullptr;
+    if (sdc_spec_.sample_interval > 0) {
+      const CorrSpec& c = sdc_spec_;
+      const int* contents = corr_groups(c, sdc_sizes);
+      const int rc = b200md_sdc_create(c.Nc, c.sample_interval, number_of_steps, time_step_,
+                                       (int)sdc_sizes.size(), sdc_sizes.data(), contents, &sdc);
+      if (rc == B200MD_ERR_ARG)
+        input_error(std::string("compute_sdc: ") + b200md_last_error());
+      if (rc != B200MD_OK)
+        b2h_fail("compute_sdc");
+    }
+    b200md_msd* msd = nullptr;
+    double msd_h[9];
+    if (msd_spec_.sample_interval > 0) {
+      const CorrSpec& c = msd_spec_;
+      const int* contents = corr_groups(c, msd_sizes);
+      const int rc = b200md_msd_create(c.Nc, c.sample_interval, number_of_steps, time_step_,
+                                       (int)msd_sizes.size(), msd_sizes.data(), contents, &msd);
+      if (rc == B200MD_ERR_ARG)
+        input_error(std::string("compute_msd: ") + b200md_last_error());
+      if (rc != B200MD_OK)
+        b2h_fail("compute_msd");
+      std::copy(model_.box.cpu_h, model_.box.cpu_h + 9, msd_h);
+      if (unwrapped_.size() < (size_t)3 * N) { // the first run with compute_msd (msd.cu:471-477)
+        unwrapped_.resize((size_t)3 * N);
+        position_old_.resize((size_t)3 * N);
+        B2H_CHECK(cudaMemcpy(unwrapped_.data(), a.position_per_atom.data(), sizeof(double) * 3 * N,
+                             cudaMemcpyDeviceToDevice));
+      }
+    }
+    const bool unwrap = unwrapped_.size() > 0;
+    const int msd_num_atoms = msd_spec_.group_method >= 0 && !msd_spec_.all_groups ? msd_sizes[0] : N;
     printf("Run %d steps.\n", number_of_steps);
     const auto t0 = std::chrono::high_resolution_clock::now();
     for (int step = 0; step < number_of_steps; ++step) {
+      if (unwrap && b200md_unwrap_begin(N, a.position_per_atom.data(), position_old_.data(), nullptr) != B200MD_OK)
+        b2h_fail("unwrapped positions");
       ensemble_->compute1(time_step_, model_.group, model_.box, a, thermo_);
+      if (unwrap && b200md_unwrap_end(N, a.position_per_atom.data(), position_old_.data(), unwrapped_.data(),
+                                      nullptr) != B200MD_OK)
+        b2h_fail("unwrapped positions");
       force_.compute(model_.box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
                      a.virial_per_atom);
       ensemble_->compute2(time_step_, model_.group, model_.box, a, thermo_);
@@ -1194,6 +1513,19 @@ private:
       if (shc && b200md_shc_sample(shc, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
                                    a.velocity_per_atom.data(), nullptr) != B200MD_OK)
         b2h_fail("compute_shc");
+      if (dos && b200md_dos_sample(dos, step, N, N, a.velocity_per_atom.data(), nullptr) != B200MD_OK)
+        b2h_fail("compute_dos");
+      if (sdc && b200md_sdc_sample(sdc, step, N, N, a.velocity_per_atom.data(), nullptr) != B200MD_OK)
+        b2h_fail("compute_sdc");
+      if (msd) {
+        if (b200md_msd_sample(msd, step, N, N, unwrapped_.data(), nullptr) != B200MD_OK)
+          b2h_fail("compute_msd");
+        const CorrSpec& c = msd_spec_; // a copy every save_every steps, on time origins (msd.cu:355-360)
+        if (c.save_every > 0 && (step + 1) % c.sample_interval == 0 && step / c.sample_interval >= c.Nc - 1 &&
+            (step + 1) % c.save_every == 0)
+          write_msd(msd, ("msd_step" + std::to_string(step + 1) + ".out").c_str(), msd_sizes, msd_num_atoms,
+                    msd_h);
+      }
       ++global_step_;
       global_time_ += time_step_;
       const bool out_thermo = fid && (step + 1) % dump_thermo_ == 0;
@@ -1246,6 +1578,18 @@ private:
     if (shc) {
       write_shc(shc, shc_groups);
       b200md_shc_destroy(shc);
+    }
+    if (dos) {
+      write_dos(dos, (int)dos_sizes.size());
+      b200md_dos_destroy(dos);
+    }
+    if (sdc) {
+      write_sdc(sdc, sdc_sizes[0]);
+      b200md_sdc_destroy(sdc);
+    }
+    if (msd) {
+      write_msd(msd, "msd.out", msd_sizes, msd_num_atoms, msd_h);
+      b200md_msd_destroy(msd);
     }
   }
 };

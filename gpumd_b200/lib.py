@@ -90,7 +90,22 @@ SIGNATURES = {
     "b200md_shc_destroy": (None, [_vp]),
     "b200md_shc_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200md_shc_finish": (C.c_int, [_vp, C.c_double, C.c_int, C.c_double, _dp, _dp, _dp, _dp, _vp]),
-    "b200md_heat_bath_create": (C.c_int, [C.c_int, C.c_int, C.c_int, _ip, _ip, C.c_int, C.c_int, C.c_double,
+    "b200md_dos_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, _ip,
+                                    _ip, C.c_int, _vp, C.POINTER(_vp)]),
+    "b200md_dos_destroy": (None, [_vp]),
+    "b200md_dos_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp]),
+    "b200md_dos_finish": (C.c_int, [_vp, _dp, _dp, _vp]),
+    "b200md_sdc_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, _ip, _ip, C.POINTER(_vp)]),
+    "b200md_sdc_destroy": (None, [_vp]),
+    "b200md_sdc_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp]),
+    "b200md_sdc_finish": (C.c_int, [_vp, _dp, _dp, _vp]),
+    "b200md_msd_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, _ip, _ip, C.POINTER(_vp)]),
+    "b200md_msd_destroy": (None, [_vp]),
+    "b200md_msd_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp]),
+    "b200md_msd_finish": (C.c_int, [_vp, _dp, _dp, _vp]),
+    "b200md_unwrap_begin": (C.c_int, [C.c_int, _vp, _vp, _vp]),
+    "b200md_unwrap_end": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp]),
+    "b200md_heat_bath_create":(C.c_int, [C.c_int, C.c_int, C.c_int, _ip, _ip, C.c_int, C.c_int, C.c_double,
                                           C.c_double, C.c_double, C.c_double, C.c_ulonglong, C.c_ulonglong,
                                           C.POINTER(_vp)]),
     "b200md_heat_bath_destroy": (None, [_vp]),

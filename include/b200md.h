@@ -304,6 +304,65 @@ int b200md_shc_finish(
   b200md_shc* p, double time_step, int num_omega, double max_omega, double* ki, double* ko,
   double* shc_i, double* shc_o, void* stream);
 
+/* Time correlations of a per-atom 3-vector over Nc lags (b2_correlate.cu):
+ *   b200md_dos_*  <- DOS (mass-weighted velocity autocorrelation, phonon DOS), src/measure/dos.cu:39-503
+ *   b200md_sdc_*  <- SDC (velocity autocorrelation, self-diffusion coefficient), src/measure/sdc.cu:34-338
+ *   b200md_msd_*  <- MSD (mean-square displacement of unwrapped positions), src/measure/msd.cu:52-542
+ * _create  <- parse + preprocess (dos.cu:153-336, sdc.cu:132-155,300-338, msd.cu:205-267,481-542).
+ *            Output groups as in b200md_shc_create: num_groups sizes and (host) contents concatenated
+ *            in Group::find_contents order; contents = NULL: one group, the atoms 0 .. group_sizes[0]-1.
+ *            `compute_dos ... group m -1` and `compute_msd ... all_groups m` pass every group of method m.
+ *            time_step in natural units.  B200MD_ERR_ARG when Nc < 1 or sample_interval < 1, for the
+ *            reference's checks (DOS: omega_max > 0, num_dos_points >= 1, the Nyquist check of
+ *            dos.cu:286-288; MSD: Nc <= number_of_steps / sample_interval, msd.cu:217-219), and -- a
+ *            deliberate divergence for DOS and SDC, where the reference divides by zero -- for a run that
+ *            gives no time origin (number_of_steps / sample_interval < Nc).  B200MD_ERR_CUDA, naming the
+ *            size, when the device ring of Nc + B - 1 frames does not fit.  DOS gathers the masses of the
+ *            groups' atoms from d_mass[n] once, here (dos.cu:326-336).
+ * _sample  <- process (dos.cu:220-245, sdc.cu:157-224, msd.cu:269-362): call every step with the
+ *            velocities (DOS, SDC) or the unwrapped positions (MSD), [3][stride] SoA.  Every
+ *            sample_interval steps the groups' vectors go into a device ring; from sample Nc - 1 on each
+ *            sample is a time origin, correlated in deferred blocks with all Nc lags.  Asynchronous.
+ * _finish  <- postprocess, FP64 on the host in the reference's order of operations; flushes the pending
+ *            origins and synchronises.  Outputs are host arrays [group][component x y z][row]:
+ *            DOS: mvac [g][3][Nc] normalised by its lag-0 value per group (dos.cu:414-427; 0 / 0 for an
+ *                 empty group, as the reference) and dos [g][3][num_dos_points] after the Hann window and
+ *                 cosine transform (dos.cu:450-481), in 1/THz per group of size N_g;
+ *            SDC: vac [g][3][Nc] in A^2/ps^2 (scaled by 1 / (N_g origins)) and its running trapezoid
+ *                 integral sdc [g][3][Nc] in A^2/ps (sdc.cu:239-285);
+ *            MSD: msd [g][3][Nc] in A^2 and the finite-difference sdc [g][3][Nc] in A^2/ps, rows of zeros
+ *                 for an empty group (msd.cu:369-445).  It may be called during the run (save_every): it
+ *                 then covers every origin sampled so far.
+ *            B200MD_ERR_ARG when no time origin has been sampled yet.
+ * b200md_unwrap_begin / _end <- Integrate::compute1, integrate.cu:347-374: call _begin before the
+ *            ensemble's first half step (copies d_position[3][n] to d_position_old) and _end after it
+ *            (d_unwrapped += d_position - d_position_old).  Wrapping into the box happens later, in the
+ *            force evaluation; a box scaling in the second half step does not reach d_unwrapped. */
+typedef struct b200md_dos b200md_dos;
+typedef struct b200md_sdc b200md_sdc;
+typedef struct b200md_msd b200md_msd;
+int b200md_dos_create(
+  int Nc, int sample_interval, int number_of_steps, double time_step, double omega_max, int num_dos_points,
+  int num_groups, const int* group_sizes, const int* contents, int n, const double* d_mass, b200md_dos** out);
+void b200md_dos_destroy(b200md_dos* p);
+int b200md_dos_sample(b200md_dos* p, int step, int n, int stride, const double* d_velocity, void* stream);
+int b200md_dos_finish(b200md_dos* p, double* mvac, double* dos, void* stream);
+int b200md_sdc_create(
+  int Nc, int sample_interval, int number_of_steps, double time_step, int num_groups,
+  const int* group_sizes, const int* contents, b200md_sdc** out);
+void b200md_sdc_destroy(b200md_sdc* p);
+int b200md_sdc_sample(b200md_sdc* p, int step, int n, int stride, const double* d_velocity, void* stream);
+int b200md_sdc_finish(b200md_sdc* p, double* vac, double* sdc, void* stream);
+int b200md_msd_create(
+  int Nc, int sample_interval, int number_of_steps, double time_step, int num_groups,
+  const int* group_sizes, const int* contents, b200md_msd** out);
+void b200md_msd_destroy(b200md_msd* p);
+int b200md_msd_sample(b200md_msd* p, int step, int n, int stride, const double* d_unwrapped, void* stream);
+int b200md_msd_finish(b200md_msd* p, double* msd, double* sdc, void* stream);
+int b200md_unwrap_begin(int n, const double* d_position, double* d_position_old, void* stream);
+int b200md_unwrap_end(
+  int n, const double* d_position, const double* d_position_old, double* d_unwrapped, void* stream);
+
 /* Direct NEMD: heat source / sink baths and group averages.
  *   b200md_heat_bath_create  <- the heat branches of the Ensemble_LAN / _NHC / _BDP constructors
  *                               (ensemble_lan.cu:43-85, ensemble_nhc.cu:52-91, ensemble_bdp.cu:50-62).

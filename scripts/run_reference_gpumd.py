@@ -38,6 +38,17 @@ NEMD_PBTE_RUN = ("ensemble nvt_ber 300 300 100\ntime_step 1\ndump_thermo 10\nrun
                  "ensemble heat_lan 300 100 20 2 5\nfix 0\nmove 1 0 0.001 0\n"
                  "compute 0 10 20 temperature jp jk\nrun 600\n")
 
+# time correlations: the graphene sheet (FP64 Tersoff) after a short nvt_ber run, and NEP Si (FP32 force
+# path) from the reference's silicon_liquid/restart1.xyz; tests/test_gpu_correlation.py runs the same inputs
+# through the b200md driver
+CORR_GRAPHENE_PRE = "ensemble nvt_ber 300 300 100\ntime_step 1\nrun 200\nensemble nve\n"
+CORR_GRAPHENE_RUNS = {
+    "dos": "compute_dos 5 100 400.0\nrun 1000\n",
+    "dos_groups": "compute_dos 5 100 400.0 group 0 -1 num_dos_points 150\nrun 1000\n",
+    "sdc_msd": "compute_sdc 2 100 group 0 3\ncompute_msd 2 100 all_groups 0 save_every 500\nrun 1000\n",
+}
+CORR_SI_RUN = "time_step 2\nensemble nve\ncompute_sdc 2 100\ncompute_msd 2 100 save_every 300\nrun 400\n"
+
 
 def write_model(path, s, symbols, vel=None):
     write_xyz(path, s, symbols, vel)
@@ -46,9 +57,10 @@ def write_model(path, s, symbols, vel=None):
 ONLY = None  # --only REGEX: run just the matching cases
 
 
-def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1):
+def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1, model_file=None):
     """gpus > 1: that many visible devices -> the reference takes its NEP_MULTIGPU path
-    (src/force/force.cu:139-160); skipped when the box has fewer."""
+    (src/force/force.cu:139-160); skipped when the box has fewer.  model_file: copy this model.xyz
+    instead of writing one from s."""
     if ONLY and not re.search(ONLY, name):
         return None, None
     import os
@@ -67,7 +79,10 @@ def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1)
     shutil.rmtree(d, ignore_errors=True)
     d.mkdir(parents=True)
     shutil.copyfile(potential, d / "potential.txt")
-    write_model(d / "model.xyz", s, symbols, vel)
+    if model_file is None:
+        write_model(d / "model.xyz", s, symbols, vel)
+    else:
+        shutil.copyfile(model_file, d / "model.xyz")
     (d / "run.in").write_text("potential potential.txt\n" + run_in)
     t0 = time.time()
     r = subprocess.run([str(BIN)], cwd=d, capture_output=True, text=True, timeout=timeout, env=env)
@@ -75,7 +90,8 @@ def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1)
     (d / "stdout.txt").write_text(r.stdout[-20000:] + "\n--- stderr ---\n" + r.stderr[-5000:])
     speed = re.findall(r"Speed of this run = ([0-9.eE+-]+) atom\*step/second", r.stdout)
     info = {"case": name, "returncode": r.returncode, "wall_s": wall,
-            "speed_atom_step_per_s": [float(x) for x in speed], "n_atoms": int(s["type"].shape[0])}
+            "speed_atom_step_per_s": [float(x) for x in speed],
+            "n_atoms": int(s["type"].shape[0]) if s is not None else None}
     (d / "model.xyz").unlink()  # large; regenerated from the seeded generators
     return d, info
 
@@ -236,6 +252,17 @@ def main():
     s["group"] = np.minimum((s["pos"][0] / s["h"][0] * 6).astype(np.int32), 5)
     vel = init_velocities(s["mass"], 300.0, seed=42)
     d, i = run_case("nemd_pbte_lan", s, pbte_sym, GOLDEN / "nep_PbTe.txt", NEMD_PBTE_RUN, vel)
+    infos.append(i)
+
+    # time correlations (outputs: mvac.out, dos.out, sdc.out, msd.out, msd_step*.out)
+    s = graphene_sheet()
+    vel = init_velocities(s["mass"], 300.0, seed=42)
+    for name, run in CORR_GRAPHENE_RUNS.items():
+        d, i = run_case(f"corr_graphene_{name}", s, ["C"], GOLDEN / "Graphene_Lindsay_2010_modified.txt",
+                        CORR_GRAPHENE_PRE + run, vel)
+        infos.append(i)
+    d, i = run_case("corr_si_sdc_msd", None, ["Si"], GOLDEN / "nep_Si_2022_NEP4_3body.txt", CORR_SI_RUN,
+                    model_file=GOLDEN / "ref_silicon_liquid_restart1.xyz")
     infos.append(i)
 
     # ---- (3) throughput at the BASELINE sizes ----
