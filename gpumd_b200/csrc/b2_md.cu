@@ -586,8 +586,11 @@ int b200md_nhc_half_step(
   cudaStream_t st = (cudaStream_t)stream;
   k_nhc_chain<<<1, 32, 0, st>>>(p->state.p, d_thermo, p->dof, p->kT, 0.5 * time_step);
   B2_LAUNCHED();
-  k_scale_by<<<grid_for(n, BLK), BLK, 0, st>>>(n, stride, p->state.p + 12, d_velocity);
-  B2_LAUNCHED();
+  // n = 0: a domain block that owns no atoms still advances its copy of the chain
+  if (n > 0) {
+    k_scale_by<<<grid_for(n, BLK), BLK, 0, st>>>(n, stride, p->state.p + 12, d_velocity);
+    B2_LAUNCHED();
+  }
   return B200MD_OK;
 }
 
@@ -635,8 +638,11 @@ int b200md_bdp_step(
   B2_LAUNCHED();
   const double* factor = reinterpret_cast<const double*>(
     reinterpret_cast<const char*>(p->state.p) + offsetof(B2BdpState, factor));
-  k_scale_by<<<grid_for(n, BLK), BLK, 0, st>>>(n, stride, factor, d_velocity);
-  B2_LAUNCHED();
+  // n = 0: a domain block that owns no atoms still draws its copy of the random numbers
+  if (n > 0) {
+    k_scale_by<<<grid_for(n, BLK), BLK, 0, st>>>(n, stride, factor, d_velocity);
+    B2_LAUNCHED();
+  }
   return B200MD_OK;
 }
 

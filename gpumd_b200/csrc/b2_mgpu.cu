@@ -743,7 +743,10 @@ int rebuild_local(Group& G)
     if (n > 0) {
       k_double_to_ll<<<grid_for(n, BLK), BLK, 0, st>>>(n, D.own_d.p + (size_t)11 * n, D.id.p); MG_COUNT();
     }
-    MG_TRY(D.pot.invalidate(s, st));
+    // a block over vacuum may hold no atoms at all: its potential keeps its old list and is not
+    // called until an exchange brings atoms in
+    if (s > 0)
+      MG_TRY(D.pot.invalidate(s, st));
     MG_TRY(D.pot.set_owned(n));
   }
   if (G.graph) { // array strides changed: the captured step is stale
@@ -802,6 +805,8 @@ int compute_force(Group& G)
 {
   for (auto& dp : G.dom) {
     Domain& D = *dp;
+    if (D.n_loc == 0)
+      continue;
     if (D.pot.kind != 0) // NEP stores its outputs (set_accumulate(0) at creation): no zeroing pass
       MG_B2(b200md_zero_properties(D.n_loc, D.pe.p, D.force.p, D.virial.p, G.stream));
     MG_TRY(D.pot.compute(D.n_loc, D.lh, D.lpbc, D.type.p, D.pos.p, D.pe.p, D.force.p, D.virial.p, G.stream));
@@ -809,7 +814,8 @@ int compute_force(Group& G)
   return B200MD_OK;
 }
 
-// partial sums over the owned atoms, then the global sum lands in every domain's thermo[]
+// partial sums over the owned atoms, then the global sum lands in every domain's thermo[]; a block
+// that owns no atoms still runs it, because its single thread block writes the zero partial
 int find_thermo(Group& G)
 {
   cudaStream_t st = G.stream;
@@ -861,8 +867,13 @@ int one_step(Group& G, double dt)
   mark(G, 0);
   if (ens == 2)
     MG_TRY(nhc_half(G, dt));
+  // blocks that own no atoms skip the per-atom launches (a zero-block grid is a launch error); the
+  // thermostat calls still run there, because they advance the chain / random state that every
+  // domain keeps a copy of and only scale when there are atoms
   for (auto& dp : G.dom) {
     Domain& D = *dp;
+    if (D.n_own == 0)
+      continue;
     MG_B2(b200md_velocity_verlet_strided(
       1, D.n_own, D.n_loc, dt, D.mass.p, D.pos.p, D.vel.p, D.force.p, st));
     // wrap only the undecomposed periodic directions (the local box is open in the others)
@@ -875,8 +886,9 @@ int one_step(Group& G, double dt)
   mark(G, 3);
   for (auto& dp : G.dom) {
     Domain& D = *dp;
-    MG_B2(b200md_velocity_verlet_strided(
-      0, D.n_own, D.n_loc, dt, D.mass.p, D.pos.p, D.vel.p, D.force.p, st));
+    if (D.n_own > 0)
+      MG_B2(b200md_velocity_verlet_strided(
+        0, D.n_own, D.n_loc, dt, D.mass.p, D.pos.p, D.vel.p, D.force.p, st));
   }
   if (ens == 2) {
     MG_TRY(nhc_half(G, dt));
@@ -884,7 +896,7 @@ int one_step(Group& G, double dt)
     MG_TRY(find_thermo(G));
     for (auto& dp : G.dom) {
       Domain& D = *dp;
-      if (ens == 1)
+      if (ens == 1 && D.n_own > 0)
         MG_B2(b200md_berendsen_temperature(
           D.n_own, D.n_loc, G.cfg.temperature, G.cfg.temperature_coupling, D.thermo.p, D.vel.p, st));
       else if (ens == 4)
@@ -1242,9 +1254,12 @@ int b200md_mgpu_heat_current(b200md_mgpu* g, double out5[5])
     const int n = D.n_own;
     MG_CUDA(D.heat.reserve(5 * (size_t)D.cap));
     MG_CUDA(D.heat5.reserve(5));
-    MG_B2(b200md_compute_heat(n, D.n_loc, D.virial.p, D.vel.p, D.heat.p, n, st));
+    if (n == 0)
+      MG_CUDA(cudaMemsetAsync(D.heat5.p, 0, 5 * sizeof(double), st));
+    else
+      MG_B2(b200md_compute_heat(n, D.n_loc, D.virial.p, D.vel.p, D.heat.p, n, st));
     // five device reductions (cub): rare call (every sample_interval steps)
-    for (int k = 0; k < 5; ++k) {
+    for (int k = 0; k < 5 && n > 0; ++k) {
       size_t need = 0;
       MG_CUDA(cub::DeviceReduce::Sum(nullptr, need, D.heat.p + (size_t)k * n, D.heat5.p + k, n, st));
       if (need > D.cub_bytes) {
@@ -1365,7 +1380,8 @@ int b200md_mgpu_profile(b200md_mgpu* g, int enable, double* ms_out, int max_out)
 int b200md_mgpu_check(b200md_mgpu* g)
 {
   for (auto& dp : g->dom)
-    MG_TRY(dp->pot.check(g->stream));
+    if (dp->n_loc > 0)
+      MG_TRY(dp->pot.check(g->stream));
   return B200MD_OK;
 }
 

@@ -369,7 +369,11 @@ B2NeighborView Neighbor::view() const
 int Neighbor::update(
   const B2Box& box, const int* d_type, const double* d_pos, int n_in, cudaStream_t st)
 {
-  if (n_in > capacity || n_in <= 0) {
+  if (n_in <= 0) {
+    set_error("no atoms: the neighbour list needs at least one");
+    return B200MD_ERR_ARG;
+  }
+  if (n_in > capacity) {
     set_error("number of atoms exceeds the capacity given at construction");
     return B200MD_ERR_ARG;
   }
@@ -487,7 +491,11 @@ int Neighbor::enable_type_tiles(int num_types)
 
 int Neighbor::invalidate(int n_new, cudaStream_t st)
 {
-  if (n_new > capacity || n_new <= 0) {
+  if (n_new <= 0) {
+    set_error("no atoms: the neighbour list needs at least one");
+    return B200MD_ERR_ARG;
+  }
+  if (n_new > capacity) {
     set_error("number of atoms exceeds the capacity given at construction");
     return B200MD_ERR_ARG;
   }

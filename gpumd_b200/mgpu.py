@@ -77,7 +77,7 @@ class DomainGroup:
         self._file = str(potential_file).encode()
         cfg.potential_file = self._file
         cfg.skin = float(skin)
-        cfg.ensemble = ENSEMBLES[ensemble]
+        cfg.ensemble = ENSEMBLES[ensemble] if isinstance(ensemble, str) else int(ensemble)  # name or C-ABI code
         cfg.temperature, cfg.temperature_coupling = float(temperature), float(temperature_coupling)
         cfg.time_step = float(time_step)
         cfg.bdp_seed = int(bdp_seed)
