@@ -15,11 +15,7 @@
 //   b200md_hnemd_drive            <- gpu_add_driving_force + gpu_sum_force + gpu_correct_force,
 //                                    src/force/force.cu:228-312, 857-897
 //   b200md_hnemd_create/_sample/_take <- HNEMD::preprocess / process, src/measure/hnemd_kappa.cu:37-132
-//   b200md_shc_create/_sample/_finish <- SHC::preprocess / process / average_k / find_shc,
-//                                    src/measure/shc.cu:34-396
-// The SHC correlation is deferred and blocked: the ring keeps Nc + SHC_B - 1 frames, and one flush
-// correlates up to SHC_B time origins with all Nc lags at once, so each ring frame is read once per
-// SHC_B origins instead of once per origin (shc.cu:249-309 reads the whole ring at every sample).
+// The spectral heat current (b200md_shc_*) runs on the correlation engine of b2_correlate.cu.
 // Every reduction has a fixed order: the results do not depend on scheduling.
 #include "../../include/b200md.h"
 #include "b2_host.h"
@@ -28,18 +24,11 @@
 #include <new>
 #include <vector>
 
-#ifndef B200MD_SHC_BLOCK
-#define B200MD_SHC_BLOCK 16
-#endif
-
 namespace b2 {
 namespace {
 
 constexpr int RED_BLK = 256;        // atoms-per-block of the ticketed reductions
 constexpr int RED_MAX_BLOCKS = 264; // two per SM of an H100 SXM
-constexpr int SHC_B = B200MD_SHC_BLOCK; // time origins per correlation flush
-constexpr int SHC_CHUNK = 256;      // atoms one warp correlates (never straddles an output group)
-constexpr int SHC_WARPS = 4;        // warps per block of k_shc_corr
 
 int red_blocks(int n)
 {
@@ -169,118 +158,6 @@ __global__ void __launch_bounds__(RED_BLK) k_hnemd_heat(
     *ticket = 0;
 }
 
-// One SHC frame: the virial row of `direction` (s_x, s_y, s_z; shc.cu:188-191) and the velocity of
-// the output groups' atoms, in Group::find_contents order (group.cu:58-70), into ring slot `frame`
-//   frame[c * G + j], c = sx sy sz vx vy vz
-__global__ void __launch_bounds__(256) k_shc_gather(
-  int G, int stride, int r0, int r1, int r2, const int* __restrict__ contents,
-  const double* __restrict__ w, const double* __restrict__ v, double* frame)
-{
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < G) {
-    const size_t s = (size_t)stride, g = (size_t)G;
-    const int m = contents ? contents[j] : j;
-    frame[j] = w[r0 * s + m];
-    frame[g + j] = w[r1 * s + m];
-    frame[2 * g + j] = w[r2 * s + m];
-    frame[3 * g + j] = v[m];
-    frame[4 * g + j] = v[s + m];
-    frame[5 * g + j] = v[2 * s + m];
-  }
-}
-
-// Blocked correlation of P <= SHC_B consecutive time origins k0 .. k0+P-1 with lags 0 .. Nc-1.
-// One warp owns one chunk (start, length) of ring atoms; blockIdx.y = 0 correlates s(now) . v(past)
-// (gpu_find_k's "negative" call), 1 correlates v(now) . s(past) ("positive").  Each lane keeps the
-// three "now" values of every origin in registers and walks the past frames f = k0+SHC_B-1 down to
-// k0-Nc+1 once: frame f adds to lag k0+p-f of origin p.  The accumulators of SHC_B consecutive lags
-// rotate through registers; after frame f the lag k0-f is complete, is reduced over the warp and
-// stored to partial[chunk][4][Nc] (c = 2*half + {in-plane x+y, out-of-plane z}).  Origins p >= P
-// carry zero "now" values.  Lags < 0 (f > k0+p) only ever reach a slot that is cleared before it
-// is stored.
-__global__ void __launch_bounds__(SHC_WARPS * 32) k_shc_corr(
-  int G, int Nc, int R, int k0, int P, int nchunks, const int2* __restrict__ chunks,
-  const double* __restrict__ ring, double* partial)
-{
-  const int lane = threadIdx.x & 31;
-  const int chunk = blockIdx.x * SHC_WARPS + (threadIdx.x >> 5);
-  if (chunk >= nchunks)
-    return; // whole warps only: no block-wide synchronisation below
-  const int half = blockIdx.y;
-  const int now_c = half == 0 ? 0 : 3, past_c = half == 0 ? 3 : 0;
-  const int2 ch = chunks[chunk];
-  double* out = partial + ((size_t)chunk * 4 + 2 * half) * Nc;
-  const size_t g = (size_t)G;
-  const int T = Nc + SHC_B - 1; // number of past frames
-  for (int sub = 0; sub < ch.y; sub += 32) {
-    const bool ok = sub + lane < ch.y;
-    const int j = ch.x + sub + lane;
-    double nx[SHC_B], ny[SHC_B], nz[SHC_B];
-#pragma unroll
-    for (int p = 0; p < SHC_B; ++p) {
-      nx[p] = ny[p] = nz[p] = 0.0;
-      if (ok && p < P) {
-        const double* fr = ring + (size_t)((k0 + p) % R) * 6 * g + now_c * g + j;
-        nx[p] = fr[0];
-        ny[p] = fr[g];
-        nz[p] = fr[2 * g];
-      }
-    }
-    double ai[SHC_B], ao[SHC_B];
-#pragma unroll
-    for (int q = 0; q < SHC_B; ++q)
-      ai[q] = ao[q] = 0.0;
-    for (int tb = 0; tb < T; tb += SHC_B) {
-#pragma unroll
-      for (int u = 0; u < SHC_B; ++u) {
-        const int t = tb + u;
-        double px = 0.0, py = 0.0, pz = 0.0;
-        if (ok && t < T) {
-          const int f = k0 + SHC_B - 1 - t; // >= k0 - Nc + 1 >= 0
-          const double* fr = ring + (size_t)(f % R) * 6 * g + past_c * g + j;
-          px = fr[0];
-          py = fr[g];
-          pz = fr[2 * g];
-        }
-#pragma unroll
-        for (int p = 0; p < SHC_B; ++p) {
-          const int q = (p + u + 1) % SHC_B; // register slot of lag p + t - (SHC_B - 1)
-          ai[q] = fma(ny[p], py, fma(nx[p], px, ai[q]));
-          ao[q] = fma(nz[p], pz, ao[q]);
-        }
-        const int q = (u + 1) % SHC_B, lag = t - (SHC_B - 1);
-        double si = ai[q], so = ao[q];
-        ai[q] = ao[q] = 0.0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          si += __shfl_down_sync(0xffffffffu, si, o);
-          so += __shfl_down_sync(0xffffffffu, so, o);
-        }
-        if (lane == 0 && lag >= 0 && lag < Nc) {
-          out[lag] = sub == 0 ? si : out[lag] + si;
-          out[Nc + lag] = sub == 0 ? so : out[Nc + lag] + so;
-        }
-      }
-    }
-  }
-}
-
-// acc[group][c][lag] += sum of partial[chunk][c][lag] over the group's chunks, in chunk order
-__global__ void __launch_bounds__(256) k_shc_reduce(
-  int ngroups, int Nc, const int* __restrict__ group_chunk, const double* __restrict__ partial,
-  double* acc)
-{
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int row = 4 * Nc;
-  if (idx >= ngroups * row)
-    return;
-  const int gr = idx / row, r = idx - gr * row;
-  double s = 0.0;
-  for (int c = group_chunk[gr]; c < group_chunk[gr + 1]; ++c)
-    s += partial[(size_t)c * row + r];
-  acc[idx] += s;
-}
-
 // one block per heat component: strided partial sums, then a tree -- the order of hac.cu:50-78
 __global__ void __launch_bounds__(1024) k_sum_heat(int n, int heat_stride, int Nd, int nd, const double* g_heat, double* g_heat_all)
 {
@@ -344,39 +221,6 @@ struct b200md_hnemd {
   DevBuf<double> heat_all; // [output_interval][5], row = step % output_interval
   DevBuf<char> scratch;    // [ticket (64 bytes)][5 * red_blocks(n) partials]
 };
-
-struct b200md_shc {
-  int Nc = 0, sample_interval = 1, direction = 0, ngroups = 0, G = 0, R = 0;
-  int max_index = -1;          // largest atom index in contents (identity: G - 1)
-  int k0 = 0, pending = 0;     // first pending time origin and how many there are
-  int num_time_origins = 0;    // shc.cu:249-251
-  int nchunks = 0;
-  DevBuf<int> contents;        // empty: the whole system in atom order
-  DevBuf<int2> chunks;         // (ring start, length) per warp
-  DevBuf<int> group_chunk;     // chunks of group g: [group_chunk[g], group_chunk[g+1])
-  DevBuf<double> ring, partial, acc;
-};
-
-namespace {
-int shc_flush(b200md_shc* p, cudaStream_t st)
-{
-  if (p->pending == 0)
-    return B200MD_OK;
-  if (p->nchunks > 0) {
-    const dim3 grid(grid_for(p->nchunks, SHC_WARPS), 2);
-    k_shc_corr<<<grid, SHC_WARPS * 32, 0, st>>>(
-      p->G, p->Nc, p->R, p->k0, p->pending, p->nchunks, p->chunks.p, p->ring.p, p->partial.p);
-    B2_LAUNCHED();
-    const int total = p->ngroups * 4 * p->Nc;
-    k_shc_reduce<<<grid_for(total, 256), 256, 0, st>>>(
-      p->ngroups, p->Nc, p->group_chunk.p, p->partial.p, p->acc.p);
-    B2_LAUNCHED();
-  }
-  p->k0 += p->pending;
-  p->pending = 0;
-  return B200MD_OK;
-}
-} // namespace
 
 extern "C" {
 
@@ -564,199 +408,6 @@ int b200md_hnemd_take(
   if (rows)
     for (size_t k = 0; k < h.size(); ++k)
       rows[k] = h[k];
-  return B200MD_OK;
-}
-
-int b200md_shc_create(
-  int Nc, int sample_interval, int direction, int number_of_steps, int num_groups,
-  const int* group_sizes, const int* contents, b200md_shc** out)
-{
-  // SHC::parse, shc.cu:466-542
-  if (!out || !group_sizes || num_groups < 1 || (!contents && num_groups != 1)) {
-    set_error("b200md_shc_create: bad argument");
-    return B200MD_ERR_ARG;
-  }
-  if (sample_interval < 1 || sample_interval > 50) {
-    set_error("b200md_shc_create: sample_interval should be in [1, 50]");
-    return B200MD_ERR_ARG;
-  }
-  if (Nc < 100 || Nc > 1000) {
-    set_error("b200md_shc_create: Nc should be in [100, 1000]");
-    return B200MD_ERR_ARG;
-  }
-  if (direction < 0 || direction > 2) {
-    set_error("b200md_shc_create: direction should be 0 (x), 1 (y) or 2 (z)");
-    return B200MD_ERR_ARG;
-  }
-  // the first time origin is sample Nc - 1; without one, average_k (shc.cu:323) divides by zero
-  if (number_of_steps / sample_interval < Nc) {
-    set_error("b200md_shc_create: the run gives no time origin (need number_of_steps / sample_interval >= Nc)");
-    return B200MD_ERR_ARG;
-  }
-  long long G = 0;
-  for (int gr = 0; gr < num_groups; ++gr) {
-    if (group_sizes[gr] < 0) {
-      set_error("b200md_shc_create: negative group size");
-      return B200MD_ERR_ARG;
-    }
-    G += group_sizes[gr];
-  }
-  if (G < 1 || G > 0x7fffffff) {
-    set_error("b200md_shc_create: the groups must hold between 1 and 2^31-1 atoms");
-    return B200MD_ERR_ARG;
-  }
-  int max_index = (int)G - 1;
-  if (contents) {
-    max_index = -1;
-    for (long long j = 0; j < G; ++j) {
-      if (contents[j] < 0) {
-        set_error("b200md_shc_create: negative atom index in contents");
-        return B200MD_ERR_ARG;
-      }
-      max_index = contents[j] > max_index ? contents[j] : max_index;
-    }
-  }
-  b200md_shc* p = new (std::nothrow) b200md_shc;
-  if (!p) {
-    set_error("out of host memory");
-    return B200MD_ERR_ARG;
-  }
-  p->Nc = Nc;
-  p->sample_interval = sample_interval;
-  p->direction = direction;
-  p->ngroups = num_groups;
-  p->G = (int)G;
-  p->R = Nc + SHC_B - 1;
-  p->max_index = max_index;
-  std::vector<int2> chunks;
-  std::vector<int> group_chunk(num_groups + 1, 0);
-  int start = 0;
-  for (int gr = 0; gr < num_groups; ++gr) {
-    group_chunk[gr] = (int)chunks.size();
-    for (int o = 0; o < group_sizes[gr]; o += SHC_CHUNK)
-      chunks.push_back(make_int2(start + o, group_sizes[gr] - o < SHC_CHUNK ? group_sizes[gr] - o : SHC_CHUNK));
-    start += group_sizes[gr];
-  }
-  group_chunk[num_groups] = (int)chunks.size();
-  p->nchunks = (int)chunks.size();
-  const bool ok =
-    p->ring.reserve((size_t)p->R * 6 * p->G) == cudaSuccess &&
-    p->partial.reserve((size_t)p->nchunks * 4 * Nc) == cudaSuccess &&
-    p->acc.reserve((size_t)num_groups * 4 * Nc) == cudaSuccess &&
-    p->chunks.reserve(chunks.size()) == cudaSuccess &&
-    p->group_chunk.reserve(group_chunk.size()) == cudaSuccess &&
-    (!contents || p->contents.reserve((size_t)G) == cudaSuccess);
-  if (!ok) {
-    cudaGetLastError(); // clear the allocation error
-    delete p;
-    set_error("out of device memory (SHC ring of Nc + " + std::to_string(SHC_B - 1) + " frames of " +
-              std::to_string(G) + " atoms)");
-    return B200MD_ERR_CUDA;
-  }
-  // the ring starts as zeros: a partial flush multiplies not-yet-written slots by zero
-  if (cudaMemset(p->ring.p, 0, sizeof(double) * p->R * 6 * (size_t)p->G) != cudaSuccess ||
-      cudaMemset(p->acc.p, 0, sizeof(double) * num_groups * 4 * (size_t)Nc) != cudaSuccess ||
-      cudaMemcpy(p->chunks.p, chunks.data(), sizeof(int2) * chunks.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(p->group_chunk.p, group_chunk.data(), sizeof(int) * group_chunk.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
-      (contents && cudaMemcpy(p->contents.p, contents, sizeof(int) * (size_t)G, cudaMemcpyHostToDevice) != cudaSuccess)) {
-    delete p;
-    set_error("b200md_shc_create: CUDA error while initialising");
-    return B200MD_ERR_CUDA;
-  }
-  *out = p;
-  return B200MD_OK;
-}
-
-void b200md_shc_destroy(b200md_shc* p) { delete p; }
-
-int b200md_shc_sample(
-  b200md_shc* p, int step, int n, int stride, const double* d_virial, const double* d_velocity,
-  void* stream)
-{
-  if (!p || step < 0 || n <= p->max_index || stride < n) {
-    set_error("b200md_shc_sample: bad argument (n must exceed every atom index of the groups)");
-    return B200MD_ERR_ARG;
-  }
-  if ((step + 1) % p->sample_interval != 0)
-    return B200MD_OK;
-  const int k = step / p->sample_interval; // sample_step, shc.cu:182
-  cudaStream_t st = (cudaStream_t)stream;
-  const int tensor[3][3] = {{0, 3, 4}, {6, 1, 5}, {7, 8, 2}}; // shc.cu:188
-  const int* t = tensor[p->direction];
-  k_shc_gather<<<grid_for(p->G, 256), 256, 0, st>>>(
-    p->G, stride, t[0], t[1], t[2], p->contents.p, d_virial, d_velocity,
-    p->ring.p + (size_t)(k % p->R) * 6 * p->G);
-  B2_LAUNCHED();
-  if (k >= p->Nc - 1) {
-    if (p->pending == 0)
-      p->k0 = k;
-    ++p->pending;
-    ++p->num_time_origins;
-    if (p->pending == SHC_B)
-      return shc_flush(p, st);
-  }
-  return B200MD_OK;
-}
-
-int b200md_shc_finish(
-  b200md_shc* p, double time_step, int num_omega, double max_omega, double* ki, double* ko,
-  double* shc_i, double* shc_o, void* stream)
-{
-  if (!p || num_omega < 0 || !(max_omega > 0.0) || !ki || !ko || (num_omega > 0 && (!shc_i || !shc_o))) {
-    set_error("b200md_shc_finish: bad argument (num_omega >= 0, max_omega > 0)");
-    return B200MD_ERR_ARG;
-  }
-  if (p->num_time_origins == 0) {
-    set_error("b200md_shc_finish: no time origin was sampled");
-    return B200MD_ERR_ARG;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const int rc = shc_flush(p, st);
-  if (rc != B200MD_OK)
-    return rc;
-  const int Nc = p->Nc, Nk = 2 * Nc - 1;
-  std::vector<double> acc((size_t)p->ngroups * 4 * Nc);
-  B2_CUDA(cudaMemcpyAsync(acc.data(), p->acc.p, sizeof(double) * acc.size(), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  const double PI = 3.14159265358979;             // common.cuh:19
-  const double TIME_UNIT_CONVERSION = 1.018051e+1; // common.cuh:26
-  const double scalar = 1000.0 / TIME_UNIT_CONVERSION / p->num_time_origins;
-  const double dt_in_ps = time_step * p->sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-  const double d_omega = max_omega / num_omega;
-  for (int gr = 0; gr < p->ngroups; ++gr) {
-    const double* a = acc.data() + (size_t)gr * 4 * Nc; // neg_i, neg_o, pos_i, pos_o
-    double* gi = ki + (size_t)gr * Nk;
-    double* go = ko + (size_t)gr * Nk;
-    for (int nc = 0; nc < Nc - 1; ++nc) { // average_k, shc.cu:312-348
-      gi[nc] = a[Nc - nc - 1] * scalar;
-      go[nc] = a[Nc + Nc - nc - 1] * scalar;
-    }
-    for (int nc = 0; nc < Nc; ++nc) {
-      gi[nc + Nc - 1] = a[2 * Nc + nc] * scalar;
-      go[nc + Nc - 1] = a[3 * Nc + nc] * scalar;
-    }
-    // find_shc, shc.cu:350-396: Hann window, then the cosine transform (the windowed ki / ko are
-    // what shc.out lists)
-    for (int nc = 0; nc < Nk; ++nc) {
-      const double hann_window = (cos(PI * (nc + 1 - Nc) / Nc) + 1.0) * 0.5;
-      gi[nc] *= hann_window;
-      go[nc] *= hann_window;
-    }
-    double* si = shc_i + (size_t)gr * num_omega;
-    double* so = shc_o + (size_t)gr * num_omega;
-    for (int nw = 0; nw < num_omega; ++nw) {
-      const double omega = (nw + 1) * d_omega;
-      double s_i = 0.0, s_o = 0.0;
-      for (int nc = 0; nc < Nk; nc++) {
-        const double t_in_ps = (nc + 1 - Nc) * dt_in_ps;
-        const double cos_factor = cos(omega * t_in_ps);
-        s_i += gi[nc] * cos_factor;
-        s_o += go[nc] * cos_factor;
-      }
-      si[nw] = s_i * 2.0 * dt_in_ps;
-      so[nw] = s_o * 2.0 * dt_in_ps;
-    }
-  }
   return B200MD_OK;
 }
 

@@ -432,49 +432,6 @@ class HNEMD:
         return kappa, rows.reshape(self.output_interval, 5)
 
 
-class SHC:
-    """compute_shc, src/measure/shc.cu.  groups: None for the whole system of num_atoms atoms, or a
-    list of int arrays, the atom indices of each output group (Group::find_contents order).
-    process(step, atom) every step; postprocess() returns ki, ko [num_groups, 2Nc-1] and shc_i, shc_o
-    [num_groups, num_omega]."""
-
-    def __init__(self, sample_interval, Nc, direction, number_of_steps, num_atoms=None, groups=None):
-        _require_cuda()
-        self._L = _lib.load()
-        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
-        if groups is None:
-            sizes, contents = np.array([int(num_atoms)], np.int32), None
-        else:
-            sizes = np.array([len(g) for g in groups], np.int32)
-            contents = np.ascontiguousarray(np.concatenate([np.asarray(g, np.int32) for g in groups]))
-        self.num_groups = sizes.shape[0]
-        ip = C.POINTER(C.c_int)
-        h = C.c_void_p()
-        _lib.check(self._L.b200md_shc_create(
-            self.Nc, self.sample_interval, int(direction), int(number_of_steps), self.num_groups,
-            sizes.ctypes.data_as(ip), None if contents is None else contents.ctypes.data_as(ip), C.byref(h)))
-        self._h = h
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            self._L.b200md_shc_destroy(self._h)
-            self._h = None
-
-    def process(self, step, atom):
-        n = atom.number_of_atoms
-        _lib.check(self._L.b200md_shc_sample(self._h, int(step), n, n, _ptr(atom.virial_per_atom),
-                                             _ptr(atom.velocity_per_atom), _stream()))
-
-    def postprocess(self, time_step, num_omega, max_omega):
-        g, nk, nw = self.num_groups, 2 * self.Nc - 1, int(num_omega)
-        ki, ko, si, so = np.zeros(g * nk), np.zeros(g * nk), np.zeros(max(g * nw, 1)), np.zeros(max(g * nw, 1))
-        dp = C.POINTER(C.c_double)
-        _lib.check(self._L.b200md_shc_finish(
-            self._h, float(time_step), nw, float(max_omega), ki.ctypes.data_as(dp), ko.ctypes.data_as(dp),
-            si.ctypes.data_as(dp), so.ctypes.data_as(dp), _stream()))
-        return ki.reshape(g, nk), ko.reshape(g, nk), si[:g * nw].reshape(g, nw), so[:g * nw].reshape(g, nw)
-
-
 def _groups_arg(num_atoms, groups):
     """(sizes, contents) of b200md_*_create: None -> the whole system in atom order."""
     if groups is None:
@@ -485,7 +442,7 @@ def _groups_arg(num_atoms, groups):
 
 
 class _Correlation:
-    """The shared shape of DOS, SDC and MSD: process(step, atom) every step, postprocess() at the end
+    """The shared shape of DOS, SDC, MSD and SHC: process(step, atom) every step, postprocess() at the end
     (or, for MSD, at any time).  groups: None for the whole system of num_atoms atoms, or a list of int
     arrays, the atom indices of each output group (Group::find_contents order)."""
     _kind = ""
@@ -516,6 +473,30 @@ class _Correlation:
         _lib.check(getattr(self._L, f"b200md_{self._kind}_finish")(
             self._h, a.ctypes.data_as(dp), b.ctypes.data_as(dp), _stream()))
         return a.reshape(self.num_groups, 3, rows_a), b.reshape(self.num_groups, 3, rows_b)
+
+
+class SHC(_Correlation):
+    """compute_shc, src/measure/shc.cu.  process(step, atom) every step; postprocess() returns ki, ko
+    [num_groups, 2Nc-1] and shc_i, shc_o [num_groups, num_omega]."""
+    _kind = "shc"
+
+    def __init__(self, sample_interval, Nc, direction, number_of_steps, num_atoms=None, groups=None):
+        self.Nc, self.sample_interval = int(Nc), int(sample_interval)
+        self._create((self.Nc, self.sample_interval, int(direction), int(number_of_steps)), num_atoms, groups)
+
+    def process(self, step, atom):
+        n = atom.number_of_atoms
+        _lib.check(self._L.b200md_shc_sample(self._h, int(step), n, n, _ptr(atom.virial_per_atom),
+                                             _ptr(atom.velocity_per_atom), _stream()))
+
+    def postprocess(self, time_step, num_omega, max_omega):
+        g, nk, nw = self.num_groups, 2 * self.Nc - 1, int(num_omega)
+        ki, ko, si, so = np.zeros(g * nk), np.zeros(g * nk), np.zeros(max(g * nw, 1)), np.zeros(max(g * nw, 1))
+        dp = C.POINTER(C.c_double)
+        _lib.check(self._L.b200md_shc_finish(
+            self._h, float(time_step), nw, float(max_omega), ki.ctypes.data_as(dp), ko.ctypes.data_as(dp),
+            si.ctypes.data_as(dp), so.ctypes.data_as(dp), _stream()))
+        return ki.reshape(g, nk), ko.reshape(g, nk), si[:g * nw].reshape(g, nw), so[:g * nw].reshape(g, nw)
 
 
 class DOS(_Correlation):

@@ -366,33 +366,29 @@ private:
   struct HacSpec {
     int interval = 0, Nc = 0, output_interval = 1;
   } hac_spec_;
-  // compute_hnemd output_interval fe_x fe_y fe_z (hnemd_kappa.cu:142-184) and compute_shc
-  // sample_interval Nc direction num_omega max_omega [group method id] (shc.cu:466-542); both are
-  // reset after each run (HNEMD::postprocess, SHC::postprocess, Force::finalize)
+  // compute_hnemd output_interval fe_x fe_y fe_z (hnemd_kappa.cu:142-184); reset after each run
+  // (HNEMD::postprocess, Force::finalize)
   struct HnemdSpec {
     int output_interval = 0; // 0: off
     double fe[3] = {0.0, 0.0, 0.0};
   } hnemd_spec_;
-  struct ShcSpec {
-    int sample_interval = 0; // 0: off
-    int Nc = 0, direction = 0, num_omega = 0, group_method = -1, group_id = 0;
-    double max_omega = 0.0;
-  } shc_spec_;
   // compute grouping_method sample_interval output_interval quantities... (compute.cu:595-660); reset
   // after each run (Compute::postprocess, :69-88)
   struct ComputeSpec {
     int grouping_method = 0, sample_interval = 0, output_interval = 0; // sample_interval 0: off
     unsigned mask = 0;
   } compute_spec_;
-  // compute_dos / compute_sdc / compute_msd (dos.cu:153-202, sdc.cu:300-338, msd.cu:481-541); reset after
-  // each run (the postprocess of each).  sample_interval 0: off; group_method -1: the whole system
+  // compute_dos / compute_sdc / compute_msd / compute_shc (dos.cu:153-202, sdc.cu:300-338,
+  // msd.cu:481-541, shc.cu:466-542); reset after each run (the postprocess of each).  sample_interval 0:
+  // off; group_method -1: the whole system
   struct CorrSpec {
     int sample_interval = 0, Nc = 0, group_method = -1, group_id = -1;
-    double omega_max = 0.0; // DOS
+    double omega_max = 0.0; // DOS, SHC (max_omega)
     int num_dos_points = -1; // DOS; -1: Nc
     bool all_groups = false; // MSD
     int save_every = -1;     // MSD
-  } dos_spec_, sdc_spec_, msd_spec_;
+    int direction = 0, num_omega = 0; // SHC
+  } dos_spec_, sdc_spec_, msd_spec_, shc_spec_;
   // atom.unwrapped_position of the reference: tracked from the first run with compute_msd on, in every
   // later run too (msd.cu:471-477, integrate.cu:347-374)
   GPU_Vector<double> unwrapped_, position_old_;
@@ -612,9 +608,8 @@ private:
       fixed_method_ = move_method_ = 0;
       hac_spec_ = HacSpec();
       hnemd_spec_ = HnemdSpec();
-      shc_spec_ = ShcSpec();
       compute_spec_ = ComputeSpec();
-      dos_spec_ = sdc_spec_ = msd_spec_ = CorrSpec();
+      dos_spec_ = sdc_spec_ = msd_spec_ = shc_spec_ = CorrSpec();
       force_.finalize();
       dump_thermo_ = 0; // non-propagating keywords are reset after each run (run.cu:329-340)
       dump_restart_ = 0;
@@ -752,7 +747,7 @@ private:
     printf("Compute SHC.\n");
     if (t.size() != 6 && t.size() != 9)
       input_error("compute_shc should have 5 or 8 parameters.");
-    ShcSpec c;
+    CorrSpec c;
     if (!valid_int(t[1], &c.sample_interval))
       input_error("Sampling interval for SHC should be an integer.");
     if (c.sample_interval < 1)
@@ -773,30 +768,21 @@ private:
       input_error("num_omega for SHC should be an integer.");
     if (c.num_omega < 0)
       input_error("num_omega for SHC should >= 0.");
-    if (!valid_real(t[5], &c.max_omega))
+    if (!valid_real(t[5], &c.omega_max))
       input_error("max_omega for SHC should be a number.");
-    if (c.max_omega <= 0)
+    if (c.omega_max <= 0)
       input_error("max_omega for SHC should > 0.");
-    if (t.size() == 9) { // parse_group(..., allow_all_groups = true), parse_utilities.cu:27-60
-      if (t[6] != "group")
+    for (size_t k = 6; k < t.size(); k++) {
+      if (t[k] != "group")
         input_error("Unrecognized argument in compute_shc.");
-      if (!valid_int(t[7], &c.group_method))
-        input_error("Grouping method should be an integer.");
-      if (c.group_method < 0)
-        input_error("Grouping method should >= 0.");
-      if (c.group_method >= (int)model_.group.size())
-        input_error("Grouping method should < number of grouping methods.");
-      if (!valid_int(t[8], &c.group_id))
-        input_error("Group ID should be an integer.");
-      if (c.group_id >= model_.group[c.group_method].number)
-        input_error("Group ID should < number of groups.");
+      parse_group(t, true, k, c);
       if (c.group_id < -1)
         input_error("group ID should >= -1 for computing SHC.");
       if (c.group_id == -1 && model_.group[c.group_method].number < 2)
         input_error("compute_shc with group ID -1 needs a grouping method with at least two groups.");
     }
     printf("    sampling interval %d, Nc %d, direction %d, num_omega %d, max_omega %g\n",
-           c.sample_interval, c.Nc, c.direction, c.num_omega, c.max_omega);
+           c.sample_interval, c.Nc, c.direction, c.num_omega, c.omega_max);
     shc_spec_ = c;
   }
 
@@ -804,20 +790,20 @@ private:
   // num_omega spectrum rows
   void write_shc(b200md_shc* shc, int num_groups)
   {
-    const ShcSpec& c = shc_spec_;
+    const CorrSpec& c = shc_spec_;
     const int Nk = 2 * c.Nc - 1;
     std::vector<double> ki((size_t)num_groups * Nk), ko(ki.size());
     std::vector<double> si((size_t)num_groups * c.num_omega + 1), so(si.size());
-    if (b200md_shc_finish(shc, time_step_, c.num_omega, c.max_omega, ki.data(), ko.data(), si.data(),
+    if (b200md_shc_finish(shc, time_step_, c.num_omega, c.omega_max, ki.data(), ko.data(), si.data(),
                           so.data(), nullptr) != B200MD_OK)
       b2h_fail("compute_shc");
     const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-    const double d_omega = c.max_omega / c.num_omega;
+    const double d_omega = c.omega_max / c.num_omega;
     FILE* fid = fopen("shc.out", "a");
     if (!fid)
       input_error("Failed to open shc.out.");
     fprintf(fid, "# compute_shc %d %d %d %d %g", c.sample_interval, c.Nc, c.direction, c.num_omega,
-            c.max_omega);
+            c.omega_max);
     if (c.group_method >= 0)
       fprintf(fid, " group %d %d", c.group_method, c.group_id);
     fprintf(fid, "\n# format_version 1\n# num_atoms %d\n", model_.atom.number_of_atoms);
@@ -970,16 +956,18 @@ private:
   }
 
   // the output groups of a correlation keyword as (sizes, contents): the whole system, one group, or
-  // every group of the method (`group m -1` for DOS, `all_groups m` for MSD)
-  const int* corr_groups(const CorrSpec& c, std::vector<int>& sizes) const
+  // every group of the method (`group m -1` for DOS, `all_groups m` for MSD), or for SHC's `group m -1`
+  // every group except 0 (shc.cu:204-205)
+  const int* corr_groups(const CorrSpec& c, std::vector<int>& sizes, bool except_group_0 = false) const
   {
     sizes.assign(1, model_.atom.number_of_atoms);
     if (c.group_method < 0)
       return nullptr; // the whole system in atom order
     const Group& g = model_.group[c.group_method];
     if (c.all_groups || c.group_id < 0) {
-      sizes = g.cpu_size;
-      return g.contents.data();
+      const int first = except_group_0 ? 1 : 0;
+      sizes.assign(g.cpu_size.begin() + first, g.cpu_size.end());
+      return g.contents.data() + g.cpu_size_sum[first]; // the groups are contiguous there
     }
     sizes.assign(1, g.cpu_size[c.group_id]);
     return g.contents.data() + g.cpu_size_sum[c.group_id];
@@ -1389,16 +1377,9 @@ private:
     b200md_shc* shc = nullptr;
     int shc_groups = 1;
     if (shc_spec_.sample_interval > 0) {
-      const ShcSpec& c = shc_spec_;
-      std::vector<int> sizes(1, a.number_of_atoms);
-      const int* contents = nullptr; // the whole system in atom order
-      if (c.group_method >= 0) {
-        const Group& g = model_.group[c.group_method];
-        const int first = c.group_id == -1 ? 1 : c.group_id; // id -1: every group except 0
-        const int last = c.group_id == -1 ? g.number - 1 : c.group_id;
-        sizes.assign(g.cpu_size.begin() + first, g.cpu_size.begin() + last + 1);
-        contents = g.contents.data() + g.cpu_size_sum[first]; // the groups are contiguous there
-      }
+      const CorrSpec& c = shc_spec_;
+      std::vector<int> sizes;
+      const int* contents = corr_groups(c, sizes, true);
       shc_groups = (int)sizes.size();
       const int rc = b200md_shc_create(c.Nc, c.sample_interval, c.direction, number_of_steps, shc_groups,
                                        sizes.data(), contents, &shc);

@@ -277,15 +277,15 @@ int b200md_hnemd_sample(
 int b200md_hnemd_take(
   b200md_hnemd* p, double volume, double temperature, double* kappa5, double* rows, void* stream);
 
-/* Spectral heat current (SHC).  Replaces SHC::parse / preprocess / process / postprocess
- * (src/measure/shc.cu:34-542):
+/* Spectral heat current (SHC), on the time-correlation engine of DOS, SDC and MSD (b2_correlate.cu,
+ * below).  Replaces SHC::parse / preprocess / process / postprocess (src/measure/shc.cu:34-542):
  *   b200md_shc_create  <- parse (:466-542) + preprocess (:34-79).  Output groups: num_groups sizes and
  *                         (host) contents, the atom indices of group 0, then group 1, ... (concatenated
  *                         in Group::find_contents order, group.cu:58-70).  contents = NULL: one group,
  *                         the atoms 0 .. group_sizes[0]-1 (no grouping).  `group m -1` passes groups
  *                         1 .. number-1 of method m.  Checks 1 <= sample_interval <= 50, 100 <= Nc <=
  *                         1000, direction 0..2, and that number_of_steps gives at least one time origin.
- *                         B200MD_ERR_CUDA when the device ring does not fit.
+ *                         B200MD_ERR_CUDA, naming the size, when the device ring does not fit.
  *   b200md_shc_sample  <- process (:162-310): call every step.  Every sample_interval steps the virial
  *                         row of `direction` and the velocities of the groups go into a device ring;
  *                         the correlation is deferred and computed for blocks of time origins
@@ -304,7 +304,7 @@ int b200md_shc_finish(
   b200md_shc* p, double time_step, int num_omega, double max_omega, double* ki, double* ko,
   double* shc_i, double* shc_o, void* stream);
 
-/* Time correlations of a per-atom 3-vector over Nc lags (b2_correlate.cu):
+/* Time correlations of a per-atom 3-vector over Nc lags, on one engine with SHC above (b2_correlate.cu):
  *   b200md_dos_*  <- DOS (mass-weighted velocity autocorrelation, phonon DOS), src/measure/dos.cu:39-503
  *   b200md_sdc_*  <- SDC (velocity autocorrelation, self-diffusion coefficient), src/measure/sdc.cu:34-338
  *   b200md_msd_*  <- MSD (mean-square displacement of unwrapped positions), src/measure/msd.cu:52-542

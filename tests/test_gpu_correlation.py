@@ -1,7 +1,7 @@
 """compute_dos / compute_sdc / compute_msd on the device: the blocked correlation kernels against the
-numpy restatement of tests/correlation_oracle.py, determinism, CUDA-graph capture, input errors, the
-unwrapped positions, and the `b200md` driver against the unmodified reference gpumd and against the
-reference's own graphene_dos and silicon_liquid results."""
+numpy restatement of tests/correlation_oracle.py, determinism, CUDA-graph capture (also of SHC, which
+runs on the same engine), input errors, the unwrapped positions, and the `b200md` driver against the
+unmodified reference gpumd and against the reference's own graphene_dos and silicon_liquid results."""
 import shutil
 import subprocess
 
@@ -150,25 +150,31 @@ def test_two_runs_are_bit_identical(eng, kind):
     assert r1[0].tobytes() == r2[0].tobytes() and r1[1].tobytes() == r2[1].tobytes()
 
 
-@pytest.mark.parametrize("kind", ["sdc", "msd"])
+@pytest.mark.parametrize("kind", ["sdc", "msd", "shc"])
 def test_sample_call_captures_into_a_cuda_graph(eng, kind):
-    """Step 34 completes the first block of 16 origins (Nc = 20), so the captured call gathers and
-    flushes; one replay equals the eager call: no host synchronisation or allocation in a sample."""
+    """The last step completes the first block of 16 origins (step 34 at Nc = 20; step 114 at SHC's
+    Nc = 100), so the captured call gathers and flushes; one replay equals the eager call: no host
+    synchronisation or allocation in a sample."""
     torch = eng.torch
-    n, Nc, steps = 2000, 20, 35
+    n, Nc = 2000, 100 if kind == "shc" else 20
+    steps = Nc + 15
     rng = np.random.default_rng(8)
     frames = [torch.as_tensor(f.reshape(-1), device="cuda") for f in rng.normal(size=(steps, 3, n))]
     atom = eng.Atom(np.zeros(n, np.int32), np.zeros((3, n)), np.ones(n))
+    if kind == "shc":
+        atom.virial_per_atom.copy_(torch.as_tensor(rng.normal(size=9 * n), device="cuda"))
 
     def make():
+        if kind == "shc":
+            return eng.SHC(1, Nc, 0, steps, num_atoms=n)
         return eng.SDC(1, Nc, steps, DT, n) if kind == "sdc" else eng.MSD(1, Nc, steps, DT, n)
 
     def call(obj, step):
-        if kind == "sdc":
+        if kind == "msd":
+            obj.process(step, frames[step])
+        else:
             atom.velocity_per_atom.copy_(frames[step])
             obj.process(step, atom)
-        else:
-            obj.process(step, frames[step])
 
     eager = make()
     for step in range(steps):
@@ -176,7 +182,7 @@ def test_sample_call_captures_into_a_cuda_graph(eng, kind):
     graphed = make()
     for step in range(steps - 1):
         call(graphed, step)
-    if kind == "sdc":
+    if kind != "msd":
         atom.velocity_per_atom.copy_(frames[steps - 1])
     torch.cuda.synchronize()
     s = torch.cuda.Stream()
@@ -184,15 +190,16 @@ def test_sample_call_captures_into_a_cuda_graph(eng, kind):
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.stream(s):
         with torch.cuda.graph(graph, stream=s):
-            if kind == "sdc":
+            if kind != "msd":
                 graphed.process(steps - 1, atom)
             else:
                 graphed.process(steps - 1, frames[steps - 1])
     torch.cuda.current_stream().wait_stream(s)
     graph.replay()
     torch.cuda.synchronize()
-    a, b = eager.postprocess(), graphed.postprocess()
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+    args = (DT, 10, 400.0) if kind == "shc" else ()
+    a, b = eager.postprocess(*args), graphed.postprocess(*args)
+    assert len(a) == len(b) and all(np.array_equal(x, y) for x, y in zip(a, b))
 
 
 def test_bad_arguments_are_rejected(eng):
@@ -222,9 +229,11 @@ def test_bad_arguments_are_rejected(eng):
 
 
 def test_out_of_memory_ring_names_its_size(eng):
-    """A ring of 1000 + 15 frames of 10^9 atoms (24 TB) cannot be allocated."""
+    """A ring of 1000 + 15 frames of 10^9 atoms (24 TB; 49 TB for SHC's six rows) cannot be allocated."""
     with pytest.raises(eng._lib.B200mdError, match="ring of Nc .* 1000000000 atoms"):
         eng.SDC(1, 1000, 1000, DT, 10**9)
+    with pytest.raises(eng._lib.B200mdError, match="shc ring of Nc .* 1000000000 atoms, 48720"):
+        eng.SHC(1, 1000, 0, 1000, num_atoms=10**9)
 
 
 def test_unwrapped_positions_across_box_crossings_and_runs(eng):
