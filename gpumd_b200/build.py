@@ -102,7 +102,7 @@ EXE = PKG / "b200md"
 def build_host(force=False):
     """The C++ host layer (adapter classes + standalone driver) -> gpumd_b200/b200md."""
     nvcc = _nvcc()
-    srcs = [HOST / f for f in ("potential.cpp", "force.cpp", "ensemble.cpp", "run.cpp")]
+    srcs = [HOST / f for f in ("potential.cpp", "force.cpp", "ensemble.cpp", "measure.cpp", "run.cpp")]
     deps = srcs + list(HOST.glob("*.h")) + [PKG.parent / "include" / "b200md.h", LIB]
     if force or _stale(EXE, deps):
         cmd = [nvcc, "-O2", "-std=c++17", "-x", "cu", "-gencode", "arch=compute_90a,code=sm_90a"] + \

@@ -20,6 +20,7 @@ public:
   // (Force::finalize, force.cu:335-339)
   void set_hnemd(const double fe[3]);
   void finalize() { hnemd_ = false; }
+  bool hnemd_on() const { return hnemd_; }
   std::vector<std::unique_ptr<Potential>> potentials;
 
 private:

@@ -7,30 +7,23 @@
 //   Run::perform_a_run (the MD loop)                src/main_gpumd/run.cu:211-341
 //   initialize_position (model.xyz)                 src/model/read_xyz.cu:145-425, 482-557
 //   Velocity::initialize                            src/main_gpumd/velocity.cu:55-75, 312-347
-//   Dump_Thermo                                     src/measure/dump_thermo.cu:57-129
-//   Dump_XYZ (extended XYZ)                         src/measure/dump_xyz.cu:68-437
-//   Dump_Restart (restart.xyz)                      src/measure/dump_restart.cu:66-140
 //   Replicate                                       src/main_gpumd/replicate.cu:20-111
-// Keywords: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
-// nvt_ber|nvt_nhc|nvt_bdp T T tau, time_step <fs>, dump_thermo <n>, dump_xyz <n> <file> [precision
-// single|double] [mass velocity force potential virial], dump_restart <n>, compute_hac, compute_hnemd,
-// compute_shc, ensemble heat_lan|heat_nhc|heat_bdp T Tc dT source sink, compute, compute_dos,
-// compute_sdc, compute_msd, run <n>.  Anything else is an input error (exit 1), as in the reference.
+// Keywords here: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
+// nvt_ber|nvt_nhc|nvt_bdp|nvt_lan|nvt_bao T T tau | npt_ber | heat_lan|heat_nhc|heat_bdp T Tc dT source
+// sink, fix, move, time_step <fs>, run <n>.  The measurement and dump keywords (dump_thermo, dump_xyz,
+// dump_restart, compute, compute_hac, compute_hnemd, compute_shc, compute_dos, compute_sdc,
+// compute_msd) are one Property each in measure.cpp, held by Measure as the reference's Measure holds
+// its properties.  Anything else is an input error (exit 1), as in the reference.
 #include "ensemble.h"
 #include "force.h"
+#include "measure.h"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
-#include <cstring>
 #include <fstream>
-#include <map>
 #include <memory>
 #include <sstream>
-
-static const double K_B = 8.617343e-5;                     // common.cuh:21
-static const double TIME_UNIT_CONVERSION = 1.018051e+1;    // common.cuh:26
-static const double PRESSURE_UNIT_CONVERSION = 1.602177e+2; // common.cuh:25
 
 #include "element_mass.h" // the reference's full MASS_TABLE (read_xyz.cu:36-142)
 
@@ -42,33 +35,6 @@ static bool element_mass(const std::string& symbol, double* mass)
       return true;
     }
   return false;
-}
-
-[[noreturn]] static void input_error(const std::string& msg)
-{
-  fprintf(stderr, "Input Error:\n    %s\n", msg.c_str());
-  exit(1);
-}
-
-// is_valid_int / is_valid_real, src/utilities/read_file.cu: the whole token must be the number
-static bool valid_int(const std::string& s, int* v)
-{
-  char* end = nullptr;
-  const long x = std::strtol(s.c_str(), &end, 10);
-  if (s.empty() || *end != '\0' || x < -2147483647L || x > 2147483647L)
-    return false;
-  *v = (int)x;
-  return true;
-}
-
-static bool valid_real(const std::string& s, double* v)
-{
-  char* end = nullptr;
-  const double x = std::strtod(s.c_str(), &end);
-  if (s.empty() || *end != '\0')
-    return false;
-  *v = x;
-  return true;
 }
 
 static std::string lower(std::string s)
@@ -92,13 +58,6 @@ static std::string header_value(const std::string& line, const std::string& key)
   const size_t q = line.find_first_of(" \t", p);
   return line.substr(p, q == std::string::npos ? std::string::npos : q - p);
 }
-
-struct Model {
-  Box box;
-  Atom atom;
-  std::vector<Group> group; // one entry per grouping method of model.xyz (group:I:k)
-  bool has_velocity = false;
-};
 
 static void read_model(const char* path, Model& m)
 {
@@ -350,52 +309,18 @@ private:
   int fixed_group_ = -1, move_group_ = -1, fixed_method_ = 0, move_method_ = 0;
   double move_velocity_[3] = {0.0, 0.0, 0.0};
   double time_step_ = 1.0 / TIME_UNIT_CONVERSION;
-  int dump_thermo_ = 0;
-  int dump_restart_ = 0;
-  // dump_xyz: interval, file, "%.9g" / "%.17g", optional per-atom columns (dump_xyz.cu:68-150)
-  struct XyzDump {
-    int interval = 0;
-    std::string file;
-    bool separated = false;
-    int precision = 2;
-    bool mass = false, velocity = false, force = false, potential = false, virial = false;
-  } dump_xyz_;
-  // compute_hac sample_interval Nc output_interval (measure/hac.cu:262-300); reset after each run
-  double hac_temperature_ = 300.0; // the temperature of the last thermostatted ensemble line (run.cu passes
-                                   // integrate.temperature2 to the measurements; an nve line leaves it)
-  struct HacSpec {
-    int interval = 0, Nc = 0, output_interval = 1;
-  } hac_spec_;
-  // compute_hnemd output_interval fe_x fe_y fe_z (hnemd_kappa.cu:142-184); reset after each run
-  // (HNEMD::postprocess, Force::finalize)
-  struct HnemdSpec {
-    int output_interval = 0; // 0: off
-    double fe[3] = {0.0, 0.0, 0.0};
-  } hnemd_spec_;
-  // compute grouping_method sample_interval output_interval quantities... (compute.cu:595-660); reset
-  // after each run (Compute::postprocess, :69-88)
-  struct ComputeSpec {
-    int grouping_method = 0, sample_interval = 0, output_interval = 0; // sample_interval 0: off
-    unsigned mask = 0;
-  } compute_spec_;
-  // compute_dos / compute_sdc / compute_msd / compute_shc (dos.cu:153-202, sdc.cu:300-338,
-  // msd.cu:481-541, shc.cu:466-542); reset after each run (the postprocess of each).  sample_interval 0:
-  // off; group_method -1: the whole system
-  struct CorrSpec {
-    int sample_interval = 0, Nc = 0, group_method = -1, group_id = -1;
-    double omega_max = 0.0; // DOS, SHC (max_omega)
-    int num_dos_points = -1; // DOS; -1: Nc
-    bool all_groups = false; // MSD
-    int save_every = -1;     // MSD
-    int direction = 0, num_omega = 0; // SHC
-  } dos_spec_, sdc_spec_, msd_spec_, shc_spec_;
+  // the temperature the measurements use: run.cu passes integrate.temperature2, the temperature of the
+  // last thermostatted ensemble line (an nve line leaves it)
+  double temperature_ = 300.0;
   // atom.unwrapped_position of the reference: tracked from the first run with compute_msd on, in every
   // later run too (msd.cu:471-477, integrate.cu:347-374)
   GPU_Vector<double> unwrapped_, position_old_;
   double global_time_ = 0.0; // natural units, as Run::global_time (run.cu:316)
   bool state_on_gpu_ = false;
   bool has_potential_ = false;
-  long global_step_ = 0;
+  Measure measure_;
+  const MeasureContext ctx_{model_,       force_,   ensemble_,    time_step_,    global_time_,
+                            temperature_, thermo_,  fixed_group_, fixed_method_, unwrapped_};
 
   void upload_state()
   {
@@ -438,6 +363,8 @@ private:
 
   void parse_one_keyword(const std::vector<std::string>& t)
   {
+    if (measure_.parse(ctx_, t))
+      return;
     Atom& a = model_.atom;
     if (t[0] == "potential") {
       if (t.size() != 2)
@@ -532,7 +459,7 @@ private:
       }
       ensemble_spec_ = e;
       if (e.type != 0)
-        hac_temperature_ = e.T;
+        temperature_ = e.T;
     } else if (t[0] == "fix") {
       // fix group_id | fix grouping_method group_id
       if (t.size() != 2 && t.size() != 3)
@@ -564,38 +491,6 @@ private:
       if (t.size() < 2)
         input_error("time_step should have at least 1 parameter.");
       time_step_ = std::atof(t[1].c_str()) / TIME_UNIT_CONVERSION; // run.cu:657
-    } else if (t[0] == "dump_thermo") {
-      if (t.size() != 2 || std::atoi(t[1].c_str()) <= 0)
-        input_error("dump_thermo should have 1 positive parameter (the interval).");
-      dump_thermo_ = std::atoi(t[1].c_str());
-    } else if (t[0] == "compute_hac") {
-      if (t.size() != 4)
-        input_error("compute_hac should have 3 parameters.");
-      hac_spec_.interval = std::atoi(t[1].c_str());
-      hac_spec_.Nc = std::atoi(t[2].c_str());
-      hac_spec_.output_interval = std::atoi(t[3].c_str());
-      if (hac_spec_.interval <= 0 || hac_spec_.Nc <= 0 || hac_spec_.output_interval <= 0)
-        input_error("compute_hac parameters should be positive integers.");
-      printf("Compute HAC.\n    sample interval is %d.\n    Nc is %d\n    output_interval is %d\n",
-             hac_spec_.interval, hac_spec_.Nc, hac_spec_.output_interval);
-    } else if (t[0] == "compute") {
-      parse_compute(t);
-    } else if (t[0] == "compute_hnemd") {
-      parse_compute_hnemd(t);
-    } else if (t[0] == "compute_shc") {
-      parse_compute_shc(t);
-    } else if (t[0] == "compute_dos") {
-      parse_compute_dos(t);
-    } else if (t[0] == "compute_sdc") {
-      parse_compute_sdc(t);
-    } else if (t[0] == "compute_msd") {
-      parse_compute_msd(t);
-    } else if (t[0] == "dump_restart") {
-      if (t.size() != 2 || std::atoi(t[1].c_str()) <= 0)
-        input_error("dump_restart should have 1 positive parameter (the interval).");
-      dump_restart_ = std::atoi(t[1].c_str());
-    } else if (t[0] == "dump_xyz") {
-      parse_dump_xyz(t);
     } else if (t[0] == "replicate") {
       if (state_on_gpu_ || has_potential_)
         input_error("replicate must come before 'potential' (run.cu:356-358).");
@@ -606,14 +501,8 @@ private:
       perform_a_run(std::atoi(t[1].c_str()));
       fixed_group_ = move_group_ = -1;
       fixed_method_ = move_method_ = 0;
-      hac_spec_ = HacSpec();
-      hnemd_spec_ = HnemdSpec();
-      compute_spec_ = ComputeSpec();
-      dos_spec_ = sdc_spec_ = msd_spec_ = shc_spec_ = CorrSpec();
+      measure_.finalize();
       force_.finalize();
-      dump_thermo_ = 0; // non-propagating keywords are reset after each run (run.cu:329-340)
-      dump_restart_ = 0;
-      dump_xyz_ = XyzDump();
     } else {
       input_error("'" + t[0] + "' is not a keyword supported by the b200md backend.");
     }
@@ -657,431 +546,6 @@ private:
            e.Tc, e.dT, e.source, e.sink);
   }
 
-  // Compute::parse, compute.cu:595-660
-  void parse_compute(const std::vector<std::string>& t)
-  {
-    printf("Compute space and/or time average of:\n");
-    if (t.size() < 5)
-      input_error("compute should have at least 4 parameters.");
-    ComputeSpec c;
-    if (!valid_int(t[1], &c.grouping_method))
-      input_error("grouping method of compute should be integer.");
-    if (c.grouping_method < 0)
-      input_error("grouping method should >= 0.");
-    if (c.grouping_method >= (int)model_.group.size())
-      input_error("grouping method exceeds the bound.");
-    if (!valid_int(t[2], &c.sample_interval))
-      input_error("sampling interval of compute should be integer.");
-    if (c.sample_interval <= 0)
-      input_error("sampling interval of compute should > 0.");
-    if (!valid_int(t[3], &c.output_interval))
-      input_error("output interval of compute should be integer.");
-    if (c.output_interval <= 0)
-      input_error("output interval of compute should > 0.");
-    static const char* names[7] = {"temperature", "potential", "force", "virial", "jp", "jk", "momentum"};
-    for (size_t k = 4; k < t.size(); ++k) {
-      int q = 0;
-      while (q < 7 && t[k] != names[q])
-        ++q;
-      if (q == 7)
-        input_error("Invalid property for compute.");
-      c.mask |= 1u << q;
-      printf("    %s\n", names[q]);
-    }
-    printf("    using grouping method %d.\n", c.grouping_method);
-    printf("    with sampling interval %d.\n", c.sample_interval);
-    printf("    and output interval %d.\n", c.output_interval);
-    compute_spec_ = c;
-  }
-
-  // Compute::output_results, compute.cu:540-561: the averages, then (with temperature) the energy
-  // transferred to the source and sink baths.  A non-heat ensemble prints 0 for both (the reference
-  // prints its never-initialised energy_transferred there).
-  void write_compute(b200md_group_compute* cp, int num_values)
-  {
-    std::vector<double> v(num_values);
-    if (b200md_group_compute_take(cp, compute_spec_.output_interval, v.data(), nullptr) != B200MD_OK)
-      b2h_fail("compute");
-    FILE* fc = fopen("compute.out", "a");
-    if (!fc)
-      input_error("Failed to open compute.out.");
-    for (double x : v)
-      fprintf(fc, "%15.6e", x);
-    if (compute_spec_.mask & B200MD_COMPUTE_TEMPERATURE) {
-      double e[2] = {0.0, 0.0};
-      if (auto* heat = dynamic_cast<Ensemble_HEAT_B200*>(ensemble_.get())) {
-        heat->read_energy_transferred();
-        e[0] = heat->b2_energy_transferred[0];
-        e[1] = heat->b2_energy_transferred[1];
-      }
-      fprintf(fc, "%15.6e%15.6e", e[0], e[1]);
-    }
-    fprintf(fc, "\n");
-    fclose(fc);
-  }
-
-  void parse_compute_hnemd(const std::vector<std::string>& t)
-  {
-    printf("Compute thermal conductivity using the HNEMD method.\n");
-    if (t.size() != 5)
-      input_error("compute_hnemd should have 4 parameters.");
-    HnemdSpec h;
-    if (!valid_int(t[1], &h.output_interval))
-      input_error("output_interval for HNEMD should be an integer number.");
-    if (h.output_interval < 1)
-      input_error("output_interval for HNEMD should be larger than 0.");
-    const char* names[3] = {"fe_x", "fe_y", "fe_z"};
-    for (int d = 0; d < 3; ++d)
-      if (!valid_real(t[2 + d], &h.fe[d]))
-        input_error(std::string(names[d]) + " for HNEMD should be a real number.");
-    if (hnemd_spec_.output_interval > 0) // Force::set_hnemd_parameters, force.cu:344-346
-      input_error("Cannot have more than one HNEMD method within one run.");
-    printf("    output_interval = %d\n    fe = (%g, %g, %g) /A\n", h.output_interval, h.fe[0], h.fe[1],
-           h.fe[2]);
-    hnemd_spec_ = h;
-    force_.set_hnemd(h.fe); // already in force for the evaluation before the loop (run.cu:217-248)
-  }
-
-  void parse_compute_shc(const std::vector<std::string>& t)
-  {
-    printf("Compute SHC.\n");
-    if (t.size() != 6 && t.size() != 9)
-      input_error("compute_shc should have 5 or 8 parameters.");
-    CorrSpec c;
-    if (!valid_int(t[1], &c.sample_interval))
-      input_error("Sampling interval for SHC should be an integer.");
-    if (c.sample_interval < 1)
-      input_error("Sampling interval for SHC should >= 1.");
-    if (c.sample_interval > 50)
-      input_error("Sampling interval for SHC should <= 50 (trust me).");
-    if (!valid_int(t[2], &c.Nc))
-      input_error("Nc for SHC should be an integer.");
-    if (c.Nc < 100)
-      input_error("Nc for SHC should >= 100 (trust me).");
-    if (c.Nc > 1000)
-      input_error("Nc for SHC should <= 1000 (trust me).");
-    if (!valid_int(t[3], &c.direction))
-      input_error("direction for SHC should be an integer.");
-    if (c.direction < 0 || c.direction > 2)
-      input_error("Transport direction should be x or y or z.");
-    if (!valid_int(t[4], &c.num_omega))
-      input_error("num_omega for SHC should be an integer.");
-    if (c.num_omega < 0)
-      input_error("num_omega for SHC should >= 0.");
-    if (!valid_real(t[5], &c.omega_max))
-      input_error("max_omega for SHC should be a number.");
-    if (c.omega_max <= 0)
-      input_error("max_omega for SHC should > 0.");
-    for (size_t k = 6; k < t.size(); k++) {
-      if (t[k] != "group")
-        input_error("Unrecognized argument in compute_shc.");
-      parse_group(t, true, k, c);
-      if (c.group_id < -1)
-        input_error("group ID should >= -1 for computing SHC.");
-      if (c.group_id == -1 && model_.group[c.group_method].number < 2)
-        input_error("compute_shc with group ID -1 needs a grouping method with at least two groups.");
-    }
-    printf("    sampling interval %d, Nc %d, direction %d, num_omega %d, max_omega %g\n",
-           c.sample_interval, c.Nc, c.direction, c.num_omega, c.omega_max);
-    shc_spec_ = c;
-  }
-
-  // SHC::postprocess, shc.cu:398-464: header, then per output group 2Nc-1 correlation rows and
-  // num_omega spectrum rows
-  void write_shc(b200md_shc* shc, int num_groups)
-  {
-    const CorrSpec& c = shc_spec_;
-    const int Nk = 2 * c.Nc - 1;
-    std::vector<double> ki((size_t)num_groups * Nk), ko(ki.size());
-    std::vector<double> si((size_t)num_groups * c.num_omega + 1), so(si.size());
-    if (b200md_shc_finish(shc, time_step_, c.num_omega, c.omega_max, ki.data(), ko.data(), si.data(),
-                          so.data(), nullptr) != B200MD_OK)
-      b2h_fail("compute_shc");
-    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-    const double d_omega = c.omega_max / c.num_omega;
-    FILE* fid = fopen("shc.out", "a");
-    if (!fid)
-      input_error("Failed to open shc.out.");
-    fprintf(fid, "# compute_shc %d %d %d %d %g", c.sample_interval, c.Nc, c.direction, c.num_omega,
-            c.omega_max);
-    if (c.group_method >= 0)
-      fprintf(fid, " group %d %d", c.group_method, c.group_id);
-    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n", model_.atom.number_of_atoms);
-    const double* h = model_.box.cpu_h;
-    fprintf(fid, "# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6],
-            h[1], h[4], h[7], h[2], h[5], h[8]);
-    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
-    fprintf(fid, "# num_correlation_rows %d\n", Nk);
-    fprintf(fid, "# num_frequency_rows %d\n", c.num_omega);
-    if (c.group_method >= 0 && c.group_id == -1)
-      fprintf(fid, "# num_output_groups %d\n", num_groups);
-    fprintf(fid, "# columns_correlation time_ps ki ko\n");
-    fprintf(fid, "# columns_shc omega_THz shc_i shc_o\n");
-    for (int g = 0; g < num_groups; ++g) {
-      for (int nc = 0; nc < Nk; ++nc) // ki, ko in A eV/ps
-        fprintf(fid, "%g %g %g\n", (nc + 1 - c.Nc) * dt_in_ps, ki[(size_t)g * Nk + nc],
-                ko[(size_t)g * Nk + nc]);
-      for (int nw = 0; nw < c.num_omega; ++nw) // shc_i, shc_o in A eV = A eV/ps/THz
-        fprintf(fid, "%g %g %g\n", (nw + 1) * d_omega, si[(size_t)g * c.num_omega + nw],
-                so[(size_t)g * c.num_omega + nw]);
-    }
-    fclose(fid);
-  }
-
-  // the sample interval and Nc that all three correlation keywords start with
-  void parse_interval_nc(const std::vector<std::string>& t, CorrSpec& c)
-  {
-    if (!valid_int(t[1], &c.sample_interval))
-      input_error("sample interval should be an integer.");
-    if (c.sample_interval <= 0)
-      input_error("sample interval should be positive.");
-    printf("    sample interval is %d.\n", c.sample_interval);
-    if (!valid_int(t[2], &c.Nc))
-      input_error("number of correlation steps should be an integer.");
-    if (c.Nc <= 0)
-      input_error("number of correlation steps should be positive.");
-    printf("    number of correlation steps is %d.\n", c.Nc);
-  }
-
-  // parse_group, src/measure/parse_utilities.cu:27-62
-  void parse_group(const std::vector<std::string>& t, bool allow_all_groups, size_t& k, CorrSpec& c)
-  {
-    if (k + 3 > t.size())
-      input_error("Not enough arguments for option 'group'.");
-    if (!valid_int(t[k + 1], &c.group_method))
-      input_error("Grouping method should be an integer.");
-    if (c.group_method < 0)
-      input_error("Grouping method should >= 0.");
-    if (c.group_method >= (int)model_.group.size())
-      input_error("Grouping method should < number of grouping methods.");
-    if (!valid_int(t[k + 2], &c.group_id))
-      input_error("Group ID should be an integer.");
-    if (c.group_id >= model_.group[c.group_method].number)
-      input_error("Group ID should < number of groups.");
-    if (c.group_id < 0 && !allow_all_groups)
-      input_error("group ID should >= 0.");
-    printf("    grouping method is %d and group ID is %d.\n", c.group_method, c.group_id);
-    k += 2;
-  }
-
-  // DOS::parse, dos.cu:153-202
-  void parse_compute_dos(const std::vector<std::string>& t)
-  {
-    printf("Compute phonon DOS.\n");
-    if (t.size() < 4)
-      input_error("compute_dos should have at least 3 parameters.");
-    if (t.size() > 9)
-      input_error("compute_dos has too many parameters.");
-    CorrSpec c;
-    parse_interval_nc(t, c);
-    if (!valid_real(t[3], &c.omega_max))
-      input_error("maximal angular frequency should be a number.");
-    if (c.omega_max <= 0)
-      input_error("maximal angular frequency should be positive.");
-    printf("    maximal angular frequency is %g THz.\n", c.omega_max);
-    for (size_t k = 4; k < t.size(); k++) {
-      if (t[k] == "group") {
-        parse_group(t, true, k, c);
-      } else if (t[k] == "num_dos_points") {
-        if (k + 2 > t.size())
-          input_error("Not enough arguments for option 'num_dos_points'.");
-        if (!valid_int(t[k + 1], &c.num_dos_points))
-          input_error("number of DOS points should be an integer.");
-        if (c.num_dos_points < 1)
-          input_error("number of DOS points must be > 0.");
-        k += 1;
-        printf("    num_dos_points is %d.\n", c.num_dos_points);
-      } else {
-        input_error("Unrecognized argument in compute_dos.");
-      }
-    }
-    dos_spec_ = c;
-  }
-
-  // SDC::parse, sdc.cu:300-338
-  void parse_compute_sdc(const std::vector<std::string>& t)
-  {
-    printf("Compute self diffusion coefficient (SDC).\n");
-    if (t.size() < 3)
-      input_error("compute_sdc should have at least 2 parameters.");
-    if (t.size() > 6)
-      input_error("compute_sdc has too many parameters.");
-    CorrSpec c;
-    parse_interval_nc(t, c);
-    for (size_t k = 3; k < t.size(); k++) {
-      if (t[k] == "group")
-        parse_group(t, false, k, c);
-      else
-        input_error("Unrecognized argument in compute_sdc.");
-    }
-    sdc_spec_ = c;
-  }
-
-  // MSD::parse, msd.cu:481-541.  all_groups reads the method after the keyword (the reference reads
-  // param[4], which is that position in the documented form `compute_msd <i> <Nc> all_groups <m>`)
-  void parse_compute_msd(const std::vector<std::string>& t)
-  {
-    printf("Compute mean square displacement (MSD).\n");
-    if (t.size() < 3)
-      input_error("compute_msd should have at least 2 parameters.");
-    if (t.size() > 8)
-      input_error("compute_msd has too many parameters.");
-    CorrSpec c;
-    parse_interval_nc(t, c);
-    for (size_t k = 3; k < t.size(); k++) {
-      if (t[k] == "group") {
-        parse_group(t, false, k, c);
-      } else if (t[k] == "all_groups") {
-        c.all_groups = true;
-        if (k + 2 > t.size() || !valid_int(t[k + 1], &c.group_method))
-          input_error("Grouping method should be an integer.");
-        if (c.group_method < 0)
-          input_error("Grouping method should >= 0.");
-        if (c.group_method >= (int)model_.group.size())
-          input_error("Grouping method should < number of grouping methods.");
-        printf("    will compute MSD for all groups in grouping %d.\n", c.group_method);
-        k += 1;
-      } else if (t[k] == "save_every") {
-        if (k + 2 > t.size() || !valid_int(t[k + 1], &c.save_every))
-          input_error("save_every should be an integer.");
-        printf("    will save a copy of the MSD every %d steps.\n", c.save_every);
-        k += 1;
-      } else {
-        input_error("Unrecognized argument in compute_msd.");
-      }
-    }
-    if (c.all_groups && c.group_method >= 0 && c.group_id >= 0)
-      input_error("Cannot compute MSD over a single group and all groups at the same time");
-    msd_spec_ = c;
-  }
-
-  // the output groups of a correlation keyword as (sizes, contents): the whole system, one group, or
-  // every group of the method (`group m -1` for DOS, `all_groups m` for MSD), or for SHC's `group m -1`
-  // every group except 0 (shc.cu:204-205)
-  const int* corr_groups(const CorrSpec& c, std::vector<int>& sizes, bool except_group_0 = false) const
-  {
-    sizes.assign(1, model_.atom.number_of_atoms);
-    if (c.group_method < 0)
-      return nullptr; // the whole system in atom order
-    const Group& g = model_.group[c.group_method];
-    if (c.all_groups || c.group_id < 0) {
-      const int first = except_group_0 ? 1 : 0;
-      sizes.assign(g.cpu_size.begin() + first, g.cpu_size.end());
-      return g.contents.data() + g.cpu_size_sum[first]; // the groups are contiguous there
-    }
-    sizes.assign(1, g.cpu_size[c.group_id]);
-    return g.contents.data() + g.cpu_size_sum[c.group_id];
-  }
-
-  // DOS::output_vac / output_dos, dos.cu:429-448,483-503: appended, no header, group after group
-  void write_dos(b200md_dos* dos, int num_groups)
-  {
-    const CorrSpec& c = dos_spec_;
-    const int Nc = c.Nc, nw = c.num_dos_points;
-    std::vector<double> mvac((size_t)num_groups * 3 * Nc), d((size_t)num_groups * 3 * nw);
-    if (b200md_dos_finish(dos, mvac.data(), d.data(), nullptr) != B200MD_OK)
-      b2h_fail("compute_dos");
-    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-    FILE* fid = fopen("mvac.out", "a");
-    if (!fid)
-      input_error("Failed to open mvac.out.");
-    for (int g = 0; g < num_groups; ++g) {
-      const double* v = mvac.data() + (size_t)g * 3 * Nc;
-      for (int nc = 0; nc < Nc; nc++)
-        fprintf(fid, "%g %g %g %g\n", nc * dt_in_ps, v[nc], v[Nc + nc], v[2 * Nc + nc]);
-    }
-    fclose(fid);
-    const double d_omega = c.omega_max / nw;
-    fid = fopen("dos.out", "a");
-    if (!fid)
-      input_error("Failed to open dos.out.");
-    for (int g = 0; g < num_groups; ++g) {
-      const double* v = d.data() + (size_t)g * 3 * nw;
-      for (int k = 0; k < nw; k++)
-        fprintf(fid, "%g %g %g %g\n", d_omega + d_omega * k, v[k], v[nw + k], v[2 * nw + k]);
-    }
-    fclose(fid);
-  }
-
-  // SDC::postprocess, sdc.cu:259-285 (the cell at the end of the run)
-  void write_sdc(b200md_sdc* sdc, int num_atoms)
-  {
-    const CorrSpec& c = sdc_spec_;
-    const int Nc = c.Nc;
-    std::vector<double> vac((size_t)3 * Nc), s((size_t)3 * Nc);
-    if (b200md_sdc_finish(sdc, vac.data(), s.data(), nullptr) != B200MD_OK)
-      b2h_fail("compute_sdc");
-    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-    FILE* fid = fopen("sdc.out", "a");
-    if (!fid)
-      input_error("Failed to open sdc.out.");
-    fprintf(fid, "# compute_sdc %d %d", c.sample_interval, Nc);
-    if (c.group_method >= 0)
-      fprintf(fid, " group %d %d", c.group_method, c.group_id);
-    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n", num_atoms);
-    const double* h = model_.box.cpu_h;
-    fprintf(fid, "# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6], h[1], h[4],
-            h[7], h[2], h[5], h[8]);
-    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
-    fprintf(fid, "# columns time_ps vacx vacy vacz sdcx sdcy sdcz\n");
-    for (int nc = 0; nc < Nc; nc++)
-      fprintf(fid, "%g %g %g %g %g %g %g\n", nc * dt_in_ps, vac[nc], vac[Nc + nc], vac[2 * Nc + nc], s[nc],
-              s[Nc + nc], s[2 * Nc + nc]);
-    fclose(fid);
-  }
-
-  // MSD::write, msd.cu:365-449; h: the cell at the start of the run (msd.cu:254-255)
-  void write_msd(b200md_msd* msd, const char* filename, const std::vector<int>& sizes, int num_atoms,
-                 const double* h)
-  {
-    const CorrSpec& c = msd_spec_;
-    const int Nc = c.Nc, ng = (int)sizes.size();
-    std::vector<double> m((size_t)ng * 3 * Nc), s(m.size());
-    if (b200md_msd_finish(msd, m.data(), s.data(), nullptr) != B200MD_OK)
-      b2h_fail("compute_msd");
-    const double dt_in_ps = time_step_ * c.sample_interval * TIME_UNIT_CONVERSION / 1000.0;
-    FILE* fid = fopen(filename, "a");
-    if (!fid)
-      input_error(std::string("Failed to open ") + filename + ".");
-    fprintf(fid, "# compute_msd %d %d", c.sample_interval, Nc);
-    if (c.all_groups)
-      fprintf(fid, " all_groups %d", c.group_method);
-    else if (c.group_method >= 0)
-      fprintf(fid, " group %d %d", c.group_method, c.group_id);
-    if (c.save_every > 0)
-      fprintf(fid, " save_every %d", c.save_every);
-    fprintf(fid, "\n# format_version 1\n# num_atoms %d\n# num_groups %d\n# num_atoms_per_group", num_atoms, ng);
-    for (int g = 0; g < ng; ++g)
-      fprintf(fid, " %d", sizes[g]);
-    fprintf(fid, "\n# cell %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e %.10e\n", h[0], h[3], h[6], h[1], h[4],
-            h[7], h[2], h[5], h[8]);
-    fprintf(fid, "# dt_output %.10e ps\n", dt_in_ps);
-    fprintf(fid, "# columns time_ps");
-    if (!c.all_groups)
-      fprintf(fid, " msdx msdy msdz sdcx sdcy sdcz");
-    else
-      for (int g = 0; g < ng; ++g)
-        fprintf(fid, " msdx_%d msdy_%d msdz_%d sdcx_%d sdcy_%d sdcz_%d", g, g, g, g, g, g);
-    fprintf(fid, "\n");
-    for (int nc = 0; nc < Nc; nc++) {
-      fprintf(fid, "%g", nc * dt_in_ps);
-      for (int g = 0; g < ng; g++) {
-        const double* a = m.data() + (size_t)g * 3 * Nc;
-        const double* b = s.data() + (size_t)g * 3 * Nc;
-        fprintf(fid, "% g %g %g %g %g %g", a[nc], a[Nc + nc], a[2 * Nc + nc], b[nc], b[Nc + nc], b[2 * Nc + nc]);
-      }
-      fprintf(fid, "\n");
-    }
-    fclose(fid);
-  }
-
-  // the temperature the measurements use: run.cu passes integrate.temperature2, which an nve line
-  // leaves at the last thermostatted value
-  double measure_temperature() const
-  {
-    return ensemble_spec_.type == 0 ? hac_temperature_ : ensemble_spec_.T;
-  }
-
   // Replicate: copies ordered a-slowest, c-fastest, atoms innermost; box columns scaled
   void replicate(const std::vector<std::string>& t)
   {
@@ -1122,330 +586,82 @@ private:
     printf("Replicate cell by %d * %d * %d.\nNumber of atoms is %d.\n", r[0], r[1], r[2], N);
   }
 
-  void parse_dump_xyz(const std::vector<std::string>& t)
+  // Integrate::initialize: a fresh ensemble object per run, from the CURRENT time step
+  void build_ensemble()
   {
-    if (t.size() < 3)
-      input_error("dump_xyz should have at least 2 parameters.");
-    XyzDump d;
-    d.interval = std::atoi(t[1].c_str());
-    if (d.interval <= 0)
-      input_error("dump interval should > 0.");
-    d.file = t[2];
-    if (d.file.back() == '*') {
-      d.separated = true;
-      d.file.pop_back();
+    const EnsembleSpec& e = ensemble_spec_;
+    if (move_group_ >= 0) { // integrate.cu:59-73
+      if (fixed_group_ < 0)
+        input_error("It is not allowed to have moving group but no fixed group.");
+      if (fixed_method_ != move_method_)
+        input_error("The fixed and moving groups must use the same grouping method.");
+      if (move_group_ == fixed_group_)
+        input_error("The fixed and moving groups cannot be the same.");
+      if (e.type != 1 && e.type != 2 && e.type != 4 && e.type != 22)
+        input_error("It is only allowed to use nvt_ber, nvt_nhc, or nvt_bdp with a moving group.");
     }
-    for (size_t m = 3; m < t.size(); ++m) {
-      if (t[m] == "precision") {
-        if (m + 1 >= t.size() || (t[m + 1] != "single" && t[m + 1] != "double"))
-          input_error("Invalid precision.");
-        d.precision = t[++m] == "single" ? 1 : 2;
-      } else if (t[m] == "mass") {
-        d.mass = true;
-      } else if (t[m] == "velocity") {
-        d.velocity = true;
-      } else if (t[m] == "force") {
-        d.force = true;
-      } else if (t[m] == "potential") {
-        d.potential = true;
-      } else if (t[m] == "virial") {
-        d.virial = true;
+    const int N = model_.atom.number_of_atoms;
+    if (e.type == 0) {
+      ensemble_.reset(new Ensemble_NVE_B200(0));
+    } else if (e.type == 1) {
+      ensemble_.reset(new Ensemble_BER_B200(1, move_group_, move_velocity_, e.T, e.Tc));
+    } else if (e.type == 4) {
+      ensemble_.reset(new Ensemble_BDP_B200(4, move_group_, move_velocity_, N, e.T, e.Tc,
+                                            e.has_seed ? e.seed : bdp_seed()));
+    } else if (e.type == 3) {
+      ensemble_.reset(new Ensemble_LAN_B200(3, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_lan.cu:39
+    } else if (e.type == 5) {
+      ensemble_.reset(new Ensemble_BAO_B200(5, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_bao.cu:39
+    } else if (e.type >= 21 && e.type <= 23) { // integrate.cu:158-199
+      const Group& g0 = model_.group[0];
+      if (e.type == 22) {
+        const unsigned long long seed_source = (unsigned long long)rand(); // ensemble_lan.cu:78-81
+        const unsigned long long seed_sink = (unsigned long long)rand();
+        ensemble_.reset(new Ensemble_HEAT_LAN_B200(22, move_group_, move_velocity_, N, g0.cpu_size,
+                                                   g0.contents.data(), e.source, e.sink, e.T, e.Tc, e.dT,
+                                                   seed_source, seed_sink));
+      } else if (e.type == 21) {
+        ensemble_.reset(new Ensemble_HEAT_NHC_B200(21, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
+                                                   e.T, e.Tc, e.dT, time_step_));
       } else {
-        input_error("Unrecognized argument in dump_xyz (supported: precision, mass, velocity, force, "
-                    "potential, virial).");
+        ensemble_.reset(new Ensemble_HEAT_BDP_B200(23, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
+                                                   e.T, e.Tc, e.dT, bdp_seed()));
       }
+    } else if (e.type == 11) {
+      const double no_rate[3] = {0, 0, 0};
+      ensemble_.reset(new Ensemble_BER_B200(11, e.T, e.Tc, e.target_p, e.num_p, e.p_coupling, 0, 0, 0, no_rate));
+    } else {
+      ensemble_.reset(new Ensemble_NHC_B200(2, move_group_, move_velocity_, N, e.T, e.Tc, time_step_));
     }
-    dump_xyz_ = d;
+    ensemble_->fixed_group = fixed_group_; // integrate.cu:279-281
+    ensemble_->fixed_grouping_method = fixed_method_;
+    ensemble_->move_grouping_method = move_method_;
   }
 
-  // one frame of extended XYZ: header keys and value formats of dump_xyz.cu:197-437
-  void write_xyz_frame(int step)
+  // the MT19937 seed of nvt_bdp and heat_bdp: the reference uses 12345678 under -DDEBUG and the clock
+  // otherwise (ensemble_bdp.cu:31-37); B200MD_DEBUG_SEED=1 selects the former for trajectory parity
+  static unsigned bdp_seed()
   {
-    const XyzDump& d = dump_xyz_;
-    Atom& a = model_.atom;
-    const Box& box = model_.box;
-    const int N = a.number_of_atoms;
-    const char* fmt = d.precision == 1 ? " %.9g" : " %.17g";
-    std::vector<double> pos((size_t)3 * N), vel, frc, pe, vir((size_t)9 * N);
-    a.position_per_atom.copy_to_host(pos.data());
-    a.virial_per_atom.copy_to_host(vir.data());
-    if (d.velocity) {
-      vel.resize((size_t)3 * N);
-      a.velocity_per_atom.copy_to_host(vel.data());
-    }
-    if (d.force) {
-      frc.resize((size_t)3 * N);
-      a.force_per_atom.copy_to_host(frc.data());
-    }
-    if (d.potential) {
-      pe.resize(N);
-      a.potential_per_atom.copy_to_host(pe.data());
-    }
-    double th[8];
-    thermo_.copy_to_host(th, 8);
-    const std::string name = d.separated ? d.file + std::to_string(step + 1) : d.file;
-    FILE* fid = fopen(name.c_str(), d.separated ? "w" : "a");
-    if (!fid)
-      input_error("Failed to open " + name + ".");
-    auto tensor = [&](const char* key, const double* v9) {
-      fprintf(fid, " %s=\"", key);
-      for (int k = 0; k < 9; ++k)
-        fprintf(fid, k == 0 ? fmt + 1 : fmt, v9[k]);
-      fprintf(fid, "\"");
-    };
-    fprintf(fid, "%d\n", N);
-    fprintf(fid, "Time=%.8f", global_time_ * TIME_UNIT_CONVERSION);
-    fprintf(fid, " pbc=\"%c %c %c\"", box.pbc_x ? 'T' : 'F', box.pbc_y ? 'T' : 'F', box.pbc_z ? 'T' : 'F');
-    const double* h = box.cpu_h;
-    const double lattice[9] = {h[0], h[3], h[6], h[1], h[4], h[7], h[2], h[5], h[8]};
-    tensor("Lattice", lattice);
-    fprintf(fid, " energy=");
-    fprintf(fid, fmt + 1, th[1]);
-    double tv[6] = {0, 0, 0, 0, 0, 0}; // totals of xx yy zz xy xz yz
-    for (int c = 0; c < 6; ++c)
-      for (int n = 0; n < N; ++n)
-        tv[c] += vir[(size_t)c * N + n];
-    const double virial[9] = {tv[0], tv[3], tv[4], tv[3], tv[1], tv[5], tv[4], tv[5], tv[2]};
-    tensor("virial", virial);
-    const double stress[9] = {th[2], th[5], th[6], th[5], th[3], th[7], th[6], th[7], th[4]};
-    tensor("stress", stress);
-    fprintf(fid, " Properties=species:S:1:pos:R:3");
-    if (d.mass)
-      fprintf(fid, ":mass:R:1");
-    if (d.velocity)
-      fprintf(fid, ":vel:R:3");
-    if (d.force)
-      fprintf(fid, ":forces:R:3");
-    if (d.potential)
-      fprintf(fid, ":energy_atom:R:1");
-    if (d.virial)
-      fprintf(fid, ":virial:R:9");
-    fprintf(fid, "\n");
-    const int vidx[9] = {0, 3, 4, 6, 1, 5, 7, 8, 2}; // GPUMD component order -> row-major 3x3
-    for (int n = 0; n < N; ++n) {
-      fprintf(fid, "%s", a.cpu_atom_symbol[n].c_str());
-      for (int k = 0; k < 3; ++k)
-        fprintf(fid, fmt, pos[n + (size_t)N * k]);
-      if (d.mass)
-        fprintf(fid, fmt, a.cpu_mass[n]);
-      if (d.velocity)
-        for (int k = 0; k < 3; ++k)
-          fprintf(fid, fmt, vel[n + (size_t)N * k] / TIME_UNIT_CONVERSION);
-      if (d.force)
-        for (int k = 0; k < 3; ++k)
-          fprintf(fid, fmt, frc[n + (size_t)N * k]);
-      if (d.potential)
-        fprintf(fid, fmt, pe[n]);
-      if (d.virial)
-        for (int k = 0; k < 9; ++k)
-          fprintf(fid, fmt, vir[n + (size_t)N * vidx[k]]);
-      fprintf(fid, "\n");
-    }
-    fclose(fid);
-  }
-
-  // restart.xyz: the model.xyz the next run can start from (dump_restart.cu:83-139)
-  void write_restart()
-  {
-    Atom& a = model_.atom;
-    const Box& box = model_.box;
-    const int N = a.number_of_atoms;
-    std::vector<double> pos((size_t)3 * N), vel((size_t)3 * N);
-    a.position_per_atom.copy_to_host(pos.data());
-    a.velocity_per_atom.copy_to_host(vel.data());
-    FILE* fid = fopen("restart.xyz", "w");
-    if (!fid)
-      input_error("Failed to open restart.xyz.");
-    const double* h = box.cpu_h;
-    fprintf(fid, "%d\n", N);
-    fprintf(fid, "pbc=\"%c %c %c\" ", box.pbc_x ? 'T' : 'F', box.pbc_y ? 'T' : 'F', box.pbc_z ? 'T' : 'F');
-    fprintf(fid, "Lattice=\"%g %g %g %g %g %g %g %g %g\" ", h[0], h[3], h[6], h[1], h[4], h[7], h[2],
-            h[5], h[8]);
-    fprintf(fid, "Properties=species:S:1:pos:R:3:mass:R:1:vel:R:3\n");
-    for (int n = 0; n < N; ++n)
-      fprintf(fid, "%s %g %g %g %g %g %g %g \n", a.cpu_atom_symbol[n].c_str(), pos[n],
-              pos[n + (size_t)N], pos[n + 2 * (size_t)N], a.cpu_mass[n],
-              vel[n] / TIME_UNIT_CONVERSION, vel[n + (size_t)N] / TIME_UNIT_CONVERSION,
-              vel[n + 2 * (size_t)N] / TIME_UNIT_CONVERSION);
-    fclose(fid);
-  }
-
-  void write_thermo(FILE* fid)
-  {
-    // dump_thermo.cu:73-129: T, K, U, then sxx syy szz syz sxz sxy in GPa, then the box
-    double th[8];
-    thermo_.copy_to_host(th, 8);
-    // the kinetic energy counts every atom but those of the fixed group (dump_thermo.cu:90-101)
-    int N = model_.atom.number_of_atoms;
-    if (fixed_group_ >= 0)
-      N -= model_.group[fixed_method_].cpu_size[fixed_group_];
-    const double* h = model_.box.cpu_h;
-    fprintf(fid, "%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e", th[0],
-            1.5 * N * K_B * th[0], th[1], th[2] * PRESSURE_UNIT_CONVERSION,
-            th[3] * PRESSURE_UNIT_CONVERSION, th[4] * PRESSURE_UNIT_CONVERSION,
-            th[7] * PRESSURE_UNIT_CONVERSION, th[6] * PRESSURE_UNIT_CONVERSION,
-            th[5] * PRESSURE_UNIT_CONVERSION);
-    fprintf(fid, "%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e%20.10e\n", h[0], h[3], h[6],
-            h[1], h[4], h[7], h[2], h[5], h[8]);
+    return std::getenv("B200MD_DEBUG_SEED") ? 12345678u
+                                            : (unsigned)std::chrono::system_clock::now().time_since_epoch().count();
   }
 
   void perform_a_run(int number_of_steps)
   {
     if (!has_potential_ || ensemble_spec_.type < 0)
       input_error("'potential' and 'ensemble' must precede 'run'.");
-    Atom& a = model_.atom;
-    { // Integrate::initialize: a fresh ensemble object per run, from the CURRENT time step
-      const EnsembleSpec& e = ensemble_spec_;
-      if (move_group_ >= 0) { // integrate.cu:59-73
-        if (fixed_group_ < 0)
-          input_error("It is not allowed to have moving group but no fixed group.");
-        if (fixed_method_ != move_method_)
-          input_error("The fixed and moving groups must use the same grouping method.");
-        if (move_group_ == fixed_group_)
-          input_error("The fixed and moving groups cannot be the same.");
-        if (e.type != 1 && e.type != 2 && e.type != 4 && e.type != 22)
-          input_error("It is only allowed to use nvt_ber, nvt_nhc, or nvt_bdp with a moving group.");
-      }
-      const int N = a.number_of_atoms;
-      if (e.type == 0) {
-        ensemble_.reset(new Ensemble_NVE_B200(0));
-      } else if (e.type == 1) {
-        ensemble_.reset(new Ensemble_BER_B200(1, move_group_, move_velocity_, e.T, e.Tc));
-      } else if (e.type == 4) {
-        // the reference seeds std::mt19937 with 12345678 under -DDEBUG and from the clock otherwise
-        // (ensemble_bdp.cu:31-37); B200MD_DEBUG_SEED=1 selects the former for trajectory parity
-        unsigned seed = e.seed;
-        if (!e.has_seed)
-          seed = std::getenv("B200MD_DEBUG_SEED")
-                   ? 12345678u
-                   : (unsigned)std::chrono::system_clock::now().time_since_epoch().count();
-        ensemble_.reset(new Ensemble_BDP_B200(4, move_group_, move_velocity_, N, e.T, e.Tc, seed));
-      } else if (e.type == 3) {
-        ensemble_.reset(new Ensemble_LAN_B200(3, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_lan.cu:39
-      } else if (e.type == 5) {
-        ensemble_.reset(new Ensemble_BAO_B200(5, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_bao.cu:39
-      } else if (e.type >= 21 && e.type <= 23) { // integrate.cu:158-199
-        const Group& g0 = model_.group[0];
-        if (e.type == 22) {
-          const unsigned long long seed_source = (unsigned long long)rand(); // ensemble_lan.cu:78-81
-          const unsigned long long seed_sink = (unsigned long long)rand();
-          ensemble_.reset(new Ensemble_HEAT_LAN_B200(22, move_group_, move_velocity_, N, g0.cpu_size,
-                                                     g0.contents.data(), e.source, e.sink, e.T, e.Tc, e.dT,
-                                                     seed_source, seed_sink));
-        } else if (e.type == 21) {
-          ensemble_.reset(new Ensemble_HEAT_NHC_B200(21, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
-                                                     e.T, e.Tc, e.dT, time_step_));
-        } else { // the B200MD_DEBUG_SEED rule of nvt_bdp (ensemble_bdp.cu:31-37)
-          const unsigned seed = std::getenv("B200MD_DEBUG_SEED")
-                                  ? 12345678u
-                                  : (unsigned)std::chrono::system_clock::now().time_since_epoch().count();
-          ensemble_.reset(new Ensemble_HEAT_BDP_B200(23, N, g0.cpu_size, g0.contents.data(), e.source, e.sink,
-                                                     e.T, e.Tc, e.dT, seed));
-        }
-      } else if (e.type == 11) {
-        const double no_rate[3] = {0, 0, 0};
-        ensemble_.reset(new Ensemble_BER_B200(11, e.T, e.Tc, e.target_p, e.num_p, e.p_coupling, 0, 0, 0, no_rate));
-      } else {
-        ensemble_.reset(new Ensemble_NHC_B200(2, move_group_, move_velocity_, N, e.T, e.Tc, time_step_));
-      }
-      ensemble_->fixed_group = fixed_group_; // integrate.cu:279-281
-      ensemble_->fixed_grouping_method = fixed_method_;
-      ensemble_->move_grouping_method = move_method_;
-    }
+    build_ensemble();
     if (!state_on_gpu_)
       upload_state();
-    FILE* fid = nullptr;
-    if (dump_thermo_ > 0) {
-      fid = fopen("thermo.out", "a");
-      fprintf(fid, "# dump_thermo %d\n# format_version 1\n# num_atoms %d\n# dt_output %.10e fs\n",
-              dump_thermo_, a.number_of_atoms, time_step_ * dump_thermo_ * TIME_UNIT_CONVERSION);
-      fprintf(fid, "# columns T KE PE sxx syy szz syz sxz sxy ax ay az bx by bz cx cy cz\n");
-    }
+    Atom& a = model_.atom;
+    const int N = a.number_of_atoms;
     // the first force evaluation is outside the timed loop, as in run.cu:217-248
     force_.compute(model_.box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
                    a.virial_per_atom);
     force_.potentials[0]->check();
-    b200md_hac* hac = nullptr;
-    if (hac_spec_.interval > 0) {
-      if (b200md_hac_create(number_of_steps, hac_spec_.interval, hac_spec_.Nc, &hac) != B200MD_OK)
-        input_error(std::string("compute_hac: ") + b200md_last_error());
-    }
-    b200md_hnemd* hnemd = nullptr;
-    if (hnemd_spec_.output_interval > 0 &&
-        b200md_hnemd_create(hnemd_spec_.output_interval, hnemd_spec_.fe, &hnemd) != B200MD_OK)
-      b2h_fail("compute_hnemd");
-    b200md_shc* shc = nullptr;
-    int shc_groups = 1;
-    if (shc_spec_.sample_interval > 0) {
-      const CorrSpec& c = shc_spec_;
-      std::vector<int> sizes;
-      const int* contents = corr_groups(c, sizes, true);
-      shc_groups = (int)sizes.size();
-      const int rc = b200md_shc_create(c.Nc, c.sample_interval, c.direction, number_of_steps, shc_groups,
-                                       sizes.data(), contents, &shc);
-      if (rc == B200MD_ERR_ARG)
-        input_error(std::string("compute_shc: ") + b200md_last_error());
-      if (rc != B200MD_OK)
-        b2h_fail("compute_shc");
-    }
-    b200md_group_compute* cp = nullptr;
-    int compute_values = 0;
-    if (compute_spec_.sample_interval > 0) { // Compute::preprocess, compute.cu:31-67
-      const Group& g = model_.group[compute_spec_.grouping_method];
-      if (b200md_group_compute_create(a.number_of_atoms, g.number, g.cpu_size.data(), g.contents.data(),
-                                      compute_spec_.mask, &cp) != B200MD_OK)
-        b2h_fail("compute");
-      compute_values = b200md_group_compute_columns(cp) * g.number;
-    }
-    // DOS::preprocess, SDC::preprocess, MSD::preprocess (dos.cu:204-218, sdc.cu:132-155, msd.cu:205-267)
-    const int N = a.number_of_atoms;
-    b200md_dos* dos = nullptr;
-    std::vector<int> dos_sizes, sdc_sizes, msd_sizes;
-    if (dos_spec_.sample_interval > 0) {
-      CorrSpec& c = dos_spec_;
-      if (c.num_dos_points < 0)
-        c.num_dos_points = c.Nc;
-      const int* contents = corr_groups(c, dos_sizes);
-      const int rc = b200md_dos_create(c.Nc, c.sample_interval, number_of_steps, time_step_, c.omega_max,
-                                       c.num_dos_points, (int)dos_sizes.size(), dos_sizes.data(), contents, N,
-                                       a.mass.data(), &dos);
-      if (rc == B200MD_ERR_ARG)
-        input_error(std::string("compute_dos: ") + b200md_last_error());
-      if (rc != B200MD_OK)
-        b2h_fail("compute_dos");
-    }
-    b200md_sdc* sdc = nullptr;
-    if (sdc_spec_.sample_interval > 0) {
-      const CorrSpec& c = sdc_spec_;
-      const int* contents = corr_groups(c, sdc_sizes);
-      const int rc = b200md_sdc_create(c.Nc, c.sample_interval, number_of_steps, time_step_,
-                                       (int)sdc_sizes.size(), sdc_sizes.data(), contents, &sdc);
-      if (rc == B200MD_ERR_ARG)
-        input_error(std::string("compute_sdc: ") + b200md_last_error());
-      if (rc != B200MD_OK)
-        b2h_fail("compute_sdc");
-    }
-    b200md_msd* msd = nullptr;
-    double msd_h[9];
-    if (msd_spec_.sample_interval > 0) {
-      const CorrSpec& c = msd_spec_;
-      const int* contents = corr_groups(c, msd_sizes);
-      const int rc = b200md_msd_create(c.Nc, c.sample_interval, number_of_steps, time_step_,
-                                       (int)msd_sizes.size(), msd_sizes.data(), contents, &msd);
-      if (rc == B200MD_ERR_ARG)
-        input_error(std::string("compute_msd: ") + b200md_last_error());
-      if (rc != B200MD_OK)
-        b2h_fail("compute_msd");
-      std::copy(model_.box.cpu_h, model_.box.cpu_h + 9, msd_h);
-      if (unwrapped_.size() < (size_t)3 * N) { // the first run with compute_msd (msd.cu:471-477)
-        unwrapped_.resize((size_t)3 * N);
-        position_old_.resize((size_t)3 * N);
-        B2H_CHECK(cudaMemcpy(unwrapped_.data(), a.position_per_atom.data(), sizeof(double) * 3 * N,
-                             cudaMemcpyDeviceToDevice));
-      }
-    }
-    const bool unwrap = unwrapped_.size() > 0;
-    const int msd_num_atoms = msd_spec_.group_method >= 0 && !msd_spec_.all_groups ? msd_sizes[0] : N;
+    measure_.preprocess(ctx_, number_of_steps);
+    const bool unwrap = unwrapped_.size() > 0; // once a measurement has started tracking them
+    position_old_.resize(unwrapped_.size());
     printf("Run %d steps.\n", number_of_steps);
     const auto t0 = std::chrono::high_resolution_clock::now();
     for (int step = 0; step < number_of_steps; ++step) {
@@ -1458,120 +674,16 @@ private:
       force_.compute(model_.box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
                      a.virial_per_atom);
       ensemble_->compute2(time_step_, model_.group, model_.box, a, thermo_);
-      if (hac && b200md_hac_sample(hac, step, a.number_of_atoms, a.number_of_atoms,
-                                   a.virial_per_atom.data(), a.velocity_per_atom.data(), nullptr) != B200MD_OK)
-        b2h_fail("compute_hac");
-      if (hnemd) {
-        if (b200md_hnemd_sample(hnemd, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
-                                a.velocity_per_atom.data(), nullptr) != B200MD_OK)
-          b2h_fail("compute_hnemd");
-        if ((step + 1) % hnemd_spec_.output_interval == 0) { // hnemd_kappa.cu:108-131
-          force_.potentials[0]->check();
-          double kappa[5];
-          if (b200md_hnemd_take(hnemd, model_.box.get_volume(), measure_temperature(), kappa, nullptr,
-                                nullptr) != B200MD_OK)
-            b2h_fail("compute_hnemd");
-          FILE* fk = fopen("kappa.out", "a");
-          if (!fk)
-            input_error("Failed to open kappa.out.");
-          for (int k = 0; k < 5; ++k)
-            fprintf(fk, "%25.15f", kappa[k]);
-          fprintf(fk, "\n");
-          fclose(fk);
-        }
-      }
-      if (cp && (step + 1) % compute_spec_.sample_interval == 0) { // Compute::process, compute.cu:351-538
-        if (b200md_group_compute_sample(cp, a.number_of_atoms, a.number_of_atoms, a.mass.data(),
-                                        a.potential_per_atom.data(), a.force_per_atom.data(),
-                                        a.virial_per_atom.data(), a.velocity_per_atom.data(),
-                                        nullptr) != B200MD_OK)
-          b2h_fail("compute");
-        if (((step + 1) / compute_spec_.sample_interval) % compute_spec_.output_interval == 0) {
-          force_.potentials[0]->check();
-          write_compute(cp, compute_values);
-        }
-      }
-      if (shc && b200md_shc_sample(shc, step, a.number_of_atoms, a.number_of_atoms, a.virial_per_atom.data(),
-                                   a.velocity_per_atom.data(), nullptr) != B200MD_OK)
-        b2h_fail("compute_shc");
-      if (dos && b200md_dos_sample(dos, step, N, N, a.velocity_per_atom.data(), nullptr) != B200MD_OK)
-        b2h_fail("compute_dos");
-      if (sdc && b200md_sdc_sample(sdc, step, N, N, a.velocity_per_atom.data(), nullptr) != B200MD_OK)
-        b2h_fail("compute_sdc");
-      if (msd) {
-        if (b200md_msd_sample(msd, step, N, N, unwrapped_.data(), nullptr) != B200MD_OK)
-          b2h_fail("compute_msd");
-        const CorrSpec& c = msd_spec_; // a copy every save_every steps, on time origins (msd.cu:355-360)
-        if (c.save_every > 0 && (step + 1) % c.sample_interval == 0 && step / c.sample_interval >= c.Nc - 1 &&
-            (step + 1) % c.save_every == 0)
-          write_msd(msd, ("msd_step" + std::to_string(step + 1) + ".out").c_str(), msd_sizes, msd_num_atoms,
-                    msd_h);
-      }
-      ++global_step_;
       global_time_ += time_step_;
-      const bool out_thermo = fid && (step + 1) % dump_thermo_ == 0;
-      const bool out_xyz = dump_xyz_.interval > 0 && (step + 1) % dump_xyz_.interval == 0;
-      const bool out_restart = dump_restart_ > 0 && (step + 1) % dump_restart_ == 0;
-      if (out_thermo || out_xyz || out_restart)
-        force_.potentials[0]->check(); // nothing computed from a truncated list reaches a file
-      if (out_thermo)
-        write_thermo(fid);
-      if (out_xyz)
-        write_xyz_frame(step);
-      if (out_restart)
-        write_restart();
+      measure_.process(ctx_, step);
     }
     B2H_CHECK(cudaDeviceSynchronize());
     force_.potentials[0]->check();
     const auto t1 = std::chrono::high_resolution_clock::now();
     const double sec = std::chrono::duration<double>(t1 - t0).count();
     printf("Time used for this run = %g second.\n", sec);
-    printf("Speed of this run = %g atom*step/second.\n", a.number_of_atoms * (double)number_of_steps / sec);
-    if (fid)
-      fclose(fid);
-    if (hac) { // HAC::postprocess, hac.cu:186-258: hac.out = t(ps), 5 hac averages, 5 rtc averages
-      const int Nc = hac_spec_.Nc, oi = hac_spec_.output_interval;
-      std::vector<double> h((size_t)5 * Nc), r((size_t)5 * Nc);
-      if (b200md_hac_finish(hac, time_step_, measure_temperature(), model_.box.get_volume(), h.data(),
-                            r.data(), nullptr) != B200MD_OK)
-        b2h_fail("compute_hac");
-      const double dt_in_ps = time_step_ * hac_spec_.interval * TIME_UNIT_CONVERSION / 1000.0;
-      FILE* fh = fopen("hac.out", "a");
-      for (int nd = 0; nd < Nc / oi; ++nd) {
-        const int nc = nd * oi;
-        fprintf(fh, "%25.15e", (nc + oi * 0.5) * dt_in_ps);
-        for (int pass = 0; pass < 2; ++pass)
-          for (int k = 0; k < 5; ++k) {
-            double ave = 0.0;
-            for (int m = 0; m < oi; ++m)
-              ave += (pass == 0 ? h : r)[(size_t)Nc * k + nc + m];
-            fprintf(fh, "%25.15e", ave / oi);
-          }
-        fprintf(fh, "\n");
-      }
-      fclose(fh);
-      b200md_hac_destroy(hac);
-    }
-    if (hnemd)
-      b200md_hnemd_destroy(hnemd);
-    if (cp)
-      b200md_group_compute_destroy(cp);
-    if (shc) {
-      write_shc(shc, shc_groups);
-      b200md_shc_destroy(shc);
-    }
-    if (dos) {
-      write_dos(dos, (int)dos_sizes.size());
-      b200md_dos_destroy(dos);
-    }
-    if (sdc) {
-      write_sdc(sdc, sdc_sizes[0]);
-      b200md_sdc_destroy(sdc);
-    }
-    if (msd) {
-      write_msd(msd, "msd.out", msd_sizes, msd_num_atoms, msd_h);
-      b200md_msd_destroy(msd);
-    }
+    printf("Speed of this run = %g atom*step/second.\n", N * (double)number_of_steps / sec);
+    measure_.postprocess(ctx_);
   }
 };
 
