@@ -285,13 +285,14 @@ __global__ void __launch_bounds__(BLK) k_replicate(
   pos_out[2 * nR + e] = pos[2 * (size_t)n + i] + a * box.h[6] + b * box.h[7] + c * box.h[8];
 }
 
-// outputs of the first replica are the outputs of the original cell (+= convention)
+// outputs of the first replica are the outputs of the original cell (+= convention, or a store with
+// overwrite); n_own > 0: atoms from n_own on keep what the caller's arrays hold
 __global__ void __launch_bounds__(BLK) k_fold_replica(
   int n, size_t nR, const double* __restrict__ acc, double* pe, double* force, double* virial,
-  int overwrite)
+  int overwrite, int n_own)
 {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n)
+  if (i >= n || (n_own > 0 && i >= n_own))
     return;
   pe[i] = (overwrite ? 0.0 : pe[i]) + acc[i];
   for (int k = 0; k < 3; ++k)
@@ -351,6 +352,10 @@ struct b200md_nep {
   // staging for the host-buffer entry point
   DevBuf<int> h_type;
   DevBuf<double> h_pos, h_out;
+  // the caller's set_accumulate / set_owned / set_active_region requests: kept here because
+  // nep_setup rebuilds the view (the supercell path grows the handle), copied into it by every compute
+  int overwrite = 0, n_own = 0, use_active = 0;
+  double act_lo[3] = {0, 0, 0}, act_hi[3] = {0, 0, 0};
   B2NepView view;
   StageProfiler prof;
   int ang_block = BLK;
@@ -1036,6 +1041,13 @@ int b200md_nep_compute(
 {
   cudaStream_t st = (cudaStream_t)stream;
   B2Box box = make_box(h, pbc);
+  p->view.overwrite = p->overwrite;
+  p->view.n_own = p->n_own;
+  p->view.use_active = p->use_active;
+  for (int d = 0; d < 3; ++d) {
+    p->view.act_lo[d] = p->act_lo[d];
+    p->view.act_hi[d] = p->act_hi[d];
+  }
   // Small periodic box (a periodic thickness <= 2.5*(rc+skin); the reference switches to explicit
   // images at 2.5*rc, nep.cu:1304-1312, nep_small_box.cuh): evaluate the smallest supercell that
   // the cell-list path accepts and keep the first replica.  Every atom of that replica sees each
@@ -1056,7 +1068,12 @@ int b200md_nep_compute(
     if (nR > p->nb.capacity) { // first small-box call (or a shrinking box): grow the scratch
       B2_CUDA(cudaStreamSynchronize(st));
       B2_TRY(nep_setup(p, nR));
+      p->view.overwrite = p->overwrite;
+      p->view.n_own = p->n_own; // supercell indices below n_own all lie in the first replica
     }
+    // The active region is in the caller's coordinates, and the image atoms of the supercell need
+    // their descriptors: a small box ignores it.
+    p->view.use_active = 0;
     B2_CUDA(p->rep_type.reserve(nR));
     B2_CUDA(p->rep_pos.reserve(3 * (size_t)nR));
     B2_CUDA(p->rep_out.reserve(13 * (size_t)nR));
@@ -1081,7 +1098,7 @@ int b200md_nep_compute(
     double* acc = p->rep_out.p;
     B2_TRY(nep_pipeline(p, box, st, acc, acc + nR, acc + 4 * (size_t)nR));
     k_fold_replica<<<grid_for(n, BLK), BLK, 0, st>>>(
-      n, (size_t)nR, acc, d_potential, d_force, d_virial, p->view.overwrite);
+      n, (size_t)nR, acc, d_potential, d_force, d_virial, p->overwrite, p->n_own);
     B2_LAUNCHED();
     return B200MD_OK;
   }
@@ -1149,28 +1166,26 @@ int b200md_nep_set_owned(b200md_nep* p, int n_owned)
     set_error("b200md_nep_set_owned: negative count");
     return B200MD_ERR_ARG;
   }
-  p->view.n_own = n_owned;
+  p->n_own = n_owned;
   return B200MD_OK;
 }
 
 int b200md_nep_set_accumulate(b200md_nep* p, int accumulate)
 {
-  p->view.overwrite = accumulate ? 0 : 1;
+  p->overwrite = accumulate ? 0 : 1;
   return B200MD_OK;
 }
 
 int b200md_nep_set_active_region(b200md_nep* p, const double lo[3], const double hi[3])
 {
-  // nep_setup (supercell path) rewrites the view: keep the request in the view only, which is what the
-  // domain module needs (its local boxes are never small boxes)
   if (!lo || !hi) {
-    p->view.use_active = 0;
+    p->use_active = 0;
     return B200MD_OK;
   }
-  p->view.use_active = 1;
+  p->use_active = 1;
   for (int d = 0; d < 3; ++d) {
-    p->view.act_lo[d] = lo[d];
-    p->view.act_hi[d] = hi[d];
+    p->act_lo[d] = lo[d];
+    p->act_hi[d] = hi[d];
   }
   return B200MD_OK;
 }

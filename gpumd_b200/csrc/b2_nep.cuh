@@ -1489,6 +1489,15 @@ B2_HD void b2_team_desc_radial(int i, int l, const B2NepView& P, const B2Box& bo
   const size_t N = (size_t)P.n;
   const B2Atom a1 = P.atoms[i];
   const int t1 = a1.type;
+  if (!b2_is_active(P, a1.x, a1.y, a1.z)) { // as in b2_body_desc_radial (uniform over the team)
+    if (l == 0) {
+      P.nn_r[i] = 0;
+      P.nn_a[i] = 0;
+    }
+    for (int n = l; n < P.nr1; n += G)
+      *b2_q_ptr(P, i, P.qt ? P.tile_slot[i] : 0, n) = 0.0f;
+    return;
+  }
   const int nn = P.nn_skin[i];
   const int* row = P.nl_skin + (size_t)i * P.skin_si;
   int* out_r = P.nl_r + (size_t)i * P.pitch_r;
@@ -1726,17 +1735,25 @@ B2_HD void b2_team_force_final(
 #pragma unroll
   for (int k = 0; k < 13; ++k)
     tot[k] = b2_team_sum(tot[k]);
-  // scatter (+=, the accumulate convention of Potential::compute): component c by lane c % G
+  // scatter (+=, the accumulate convention of Potential::compute, or a store when P.overwrite is
+  // set, as in b2_body_force_final): component c by lane c % G
   const int dst = P.perm[i];
 #pragma unroll
   for (int c = 0; c < 13; ++c) {
     if (c % G == l) {
-      if (c == 0)
-        pe[dst] += P.acc[i] + (double)tot[0]; // acc[i] = site energy from the MLP pass
-      else if (c < 4)
-        force[(size_t)(c - 1) * N + dst] += (double)tot[c];
-      else
-        virial[(size_t)(c - 4) * N + dst] += (double)tot[c];
+      double* out;
+      double val;
+      if (c == 0) {
+        out = &pe[dst];
+        val = P.acc[i] + (double)tot[0]; // acc[i] = site energy from the MLP pass
+      } else if (c < 4) {
+        out = &force[(size_t)(c - 1) * N + dst];
+        val = (double)tot[c];
+      } else {
+        out = &virial[(size_t)(c - 4) * N + dst];
+        val = (double)tot[c];
+      }
+      *out = P.overwrite ? val : *out + val;
     }
   }
 }

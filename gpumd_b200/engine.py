@@ -138,6 +138,14 @@ class NEP(Potential):
         """Spatial domains: only caller indices < n_owned get outputs (0 = all)."""
         _lib.check(self._L.b200md_nep_set_owned(self._h, int(n_owned)))
 
+    def set_active_region(self, lo=None, hi=None):
+        """Spatial domains: atoms outside [lo, hi) only serve as neighbours (None = no region)."""
+        if lo is None or hi is None:
+            _lib.check(self._L.b200md_nep_set_active_region(self._h, None, None))
+            return
+        lo, hi = ((C.c_double * 3)(*[float(x) for x in v]) for v in (lo, hi))
+        _lib.check(self._L.b200md_nep_set_active_region(self._h, lo, hi))
+
     @property
     def num_rebuilds(self):
         return self._L.b200md_nep_info(self._h, 6)

@@ -488,14 +488,18 @@ int b200md_nep_set_owned(b200md_nep* p, int n_owned);
 /* accumulate = 1 (default): outputs are ADDED to the caller's arrays, the contract of Potential::compute
  * (nep.cu:653,755-770; Force::compute zeroes them first, force.cu:794-801).  accumulate = 0: they are
  * OVERWRITTEN, so a driver with a single potential can drop its zeroing pass and the final kernel its
- * read-modify-write (208 bytes per atom and step).  Small boxes (supercell path) always accumulate. */
+ * read-modify-write (208 bytes per atom and step).  The setting, like set_owned and
+ * set_active_region, holds for every later call on the handle, small boxes (supercell path) and
+ * changes of the atom count included. */
 int b200md_nep_set_accumulate(b200md_nep* p, int accumulate);
 /* Atoms whose position (in the coordinates passed to b200md_nep_compute) lies outside [lo, hi) get
  * EMPTY radial / angular neighbour sets from the following calls: no descriptor, dU/dq or partial-
  * force work is spent on them, they only serve as neighbours of the others.  A spatial domain sets
  * this to its owned region grown by rc + skin: ghosts further away cannot be a neighbour of an owned
  * atom, so nothing an owned atom's force depends on is skipped (the reference recomputes descriptors
- * for its whole ghost layer, nep_multigpu.cu:1476-1545).  lo = hi = NULL switches it off. */
+ * for its whole ghost layer, nep_multigpu.cu:1476-1545).  lo = hi = NULL switches it off.  A small
+ * periodic box (supercell path of b200md_nep_compute) ignores the region: the image atoms of its
+ * supercell lie outside the caller's coordinates and need their descriptors. */
 int b200md_nep_set_active_region(b200md_nep* p, const double lo[3], const double hi[3]);
 
 /* ---------------------------------------------------------------------------------------------

@@ -180,6 +180,7 @@ struct emu_nep {
   bool rev_slot = false;
   std::vector<int> aslot, nla_rs;
   int n_cell = 0;                        // atoms of the caller's cell (n > n_cell: supercell)
+  int overwrite = 0, n_own = 0;          // b200md_nep_set_accumulate(p, 0) / set_owned requests
 };
 
 template <int K1>
@@ -379,11 +380,15 @@ int emu_nep_compute(
   if (R == 1) {
     if (p->n != n)
       emu_nep_alloc(p, n);
+    p->P.overwrite = p->overwrite;
+    p->P.n_own = p->n_own;
     return emu_nep_pipeline(p, box, type, pos, pe, force, virial);
   }
   const int nR = n * R;
   if (p->n != nR)
     emu_nep_alloc(p, nR);
+  p->P.overwrite = p->overwrite;
+  p->P.n_own = p->n_own;
   std::vector<int> t2(nR);
   std::vector<double> x2((size_t)3 * nR), out((size_t)13 * nR, 0.0);
   for (int r = 0; r < R; ++r) {
@@ -403,14 +408,25 @@ int emu_nep_compute(
   box = make_box(hs, pbc);
   const int rc = emu_nep_pipeline(
     p, box, t2.data(), x2.data(), out.data(), out.data() + nR, out.data() + 4 * (size_t)nR);
-  for (int i = 0; i < n; ++i) {
-    pe[i] += out[i];
+  // k_fold_replica
+  const int w = p->overwrite;
+  const int n_fold = p->n_own > 0 && p->n_own < n ? p->n_own : n;
+  for (int i = 0; i < n_fold; ++i) {
+    pe[i] = (w ? 0.0 : pe[i]) + out[i];
     for (int k = 0; k < 3; ++k)
-      force[(size_t)k * n + i] += out[nR + (size_t)k * nR + i];
+      force[(size_t)k * n + i] = (w ? 0.0 : force[(size_t)k * n + i]) + out[nR + (size_t)k * nR + i];
     for (int k = 0; k < 9; ++k)
-      virial[(size_t)k * n + i] += out[4 * (size_t)nR + (size_t)k * nR + i];
+      virial[(size_t)k * n + i] =
+        (w ? 0.0 : virial[(size_t)k * n + i]) + out[4 * (size_t)nR + (size_t)k * nR + i];
   }
   return rc;
+}
+
+// b200md_nep_set_accumulate(p, !overwrite) and b200md_nep_set_owned(p, n_own)
+void emu_nep_set_mode(emu_nep* p, int overwrite, int n_own)
+{
+  p->overwrite = overwrite;
+  p->n_own = n_own;
 }
 }
 

@@ -29,15 +29,20 @@ class EmuNep:
             self.E.emu_nep_destroy(self.h)
             self.h = None
 
-    def compute(self, type_, h, pbc, pos):
+    def compute(self, type_, h, pbc, pos, prefill=(0.0, 0.0, 0.0)):
+        """prefill: the values pe / force / virial hold before the call (accumulate mode adds to them)."""
         n = self.n
-        pe, f, v = np.zeros(n), np.zeros(3 * n), np.zeros(9 * n)
+        pe, f, v = np.full(n, prefill[0]), np.full(3 * n, prefill[1]), np.full(9 * n, prefill[2])
         ty = np.ascontiguousarray(type_, np.int32)
         p = np.ascontiguousarray(pos, np.float64).reshape(-1)
         hh = np.ascontiguousarray(h, np.float64).reshape(9)
         pb = np.ascontiguousarray(pbc, np.int32)
         rc = self.E.emu_nep_compute(self.h, n, _d(hh), _i(pb), _i(ty), _d(p), _d(pe), _d(f), _d(v))
         return rc, dict(pe=pe, force=f.reshape(3, n), virial=v.reshape(9, n))
+
+    def set_mode(self, accumulate=True, n_owned=0):
+        """b200md_nep_set_accumulate / b200md_nep_set_owned"""
+        self.E.emu_nep_set_mode(self.h, 0 if accumulate else 1, int(n_owned))
 
     def neighbors(self, mn_r, mn_a):
         n = self.n
@@ -145,6 +150,7 @@ class Emu:
         E.emu_nep_export_neighbors.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int, _ip, _ip]
         E.emu_nep_export_skin.argtypes = [C.c_void_p, C.c_int, _ip, _ip]
         E.emu_nep_export_descriptors.argtypes = [C.c_void_p, _fp]
+        E.emu_nep_set_mode.argtypes = [C.c_void_p, C.c_int, C.c_int]
         E.emu_lj_create.restype = C.c_void_p
         E.emu_lj_create.argtypes = [C.c_int, _dp, C.c_int]
         E.emu_lj_destroy.argtypes = [C.c_void_p]

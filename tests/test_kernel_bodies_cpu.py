@@ -118,6 +118,47 @@ def test_nep_accumulates_into_outputs(oracle, emu):
     assert np.array_equal(a["force"], b["force"]) and np.array_equal(a["pe"], b["pe"])
 
 
+def _store_mode_cases():
+    from cases import NEP_SMALL_CASES
+    from test_few_species_cpu import FEW_SPECIES_CASES
+    return {"PbTe": NEP_CASES["PbTe"], "zbl_k17": FEW_SPECIES_CASES["zbl_k17"], "BaZrO3": NEP_CASES["BaZrO3"],
+            "PbTe_C1": NEP_SMALL_CASES["PbTe_C1"]}
+
+
+@pytest.mark.parametrize("team", ["0", "1"])
+@pytest.mark.parametrize("case", ["PbTe", "zbl_k17", "BaZrO3", "PbTe_C1"])
+def test_final_bodies_store_mode_and_owned_range(emu, case, team, monkeypatch):
+    """b200md_nep_set_accumulate(p, 0) on the final bodies (thread per atom with one, two and many types; the
+    lane-team bodies for one and two types; the supercell fold of a small box): outputs prefilled with NaN
+    must come out equal to accumulate mode on zeros.  With set_owned(m) only atoms below m are written, in
+    both modes; accumulate mode adds to the prefill."""
+    monkeypatch.setenv("B200MD_NEP_TEAM", team)
+    model, make = _store_mode_cases()[case]
+    s = make()
+    n = s["type"].shape[0]
+    args = (s["type"], s["h"], s["pbc"], s["pos"])
+    dev = emu.nep(GOLDEN / model, n)
+    _, ref = dev.compute(*args)
+    assert all(np.isfinite(ref[k]).all() for k in ref)
+    dev.set_mode(accumulate=False)
+    for _ in range(2):  # a second store on the same handle
+        _, out = dev.compute(*args, prefill=(np.nan,) * 3)
+        for k in ("pe", "force", "virial"):
+            assert np.array_equal(out[k], ref[k]), k
+    m = 129 if n > 129 else n - 1
+    for accumulate, fill in ((False, (7.0, 7.0, 7.0)), (True, (1.0, 2.0, 3.0))):
+        dev.set_mode(accumulate=accumulate, n_owned=m)
+        _, out = dev.compute(*args, prefill=fill)
+        for k, f in zip(("pe", "force", "virial"), fill):
+            want = ref[k][..., :m] + f if accumulate else ref[k][..., :m]
+            assert np.array_equal(out[k][..., :m], want), (k, accumulate)
+            assert np.all(out[k][..., m:] == f), (k, accumulate)
+    dev.set_mode(accumulate=False, n_owned=0)
+    _, out = dev.compute(*args, prefill=(np.nan,) * 3)
+    for k in ("pe", "force", "virial"):
+        assert np.array_equal(out[k], ref[k]), k
+
+
 def test_skin_list_reuse_and_rebuild(oracle, emu):
     """Move atoms by less than skin/2: no rebuild, sets still exact.  Move one atom further:
     the predicated rebuild fires and the sets are exact again."""
