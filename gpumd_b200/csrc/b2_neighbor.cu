@@ -68,11 +68,12 @@ __global__ void __launch_bounds__(BLK) k_cell_count(B2NeighborView v, B2Box box,
   }
 }
 
-// single-block exclusive scan over the cell counts: tiles of 1024*4 with a running carry
-__global__ void __launch_bounds__(1024) k_scan_cells(B2NeighborView v, int ncell)
+// single-block (1024 threads) exclusive scan of in(0 .. count-1) into out[0 .. count]: tiles of 1024*4
+// with a running carry
+template <class In>
+__device__ __forceinline__ void block_scan_1024(int count, int* out, In in)
 {
-  if (!v.flags[0])
-    return;
+  const int ncell = count;
   __shared__ int warp_sums[32];
   __shared__ int carry_s;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -84,7 +85,7 @@ __global__ void __launch_bounds__(1024) k_scan_cells(B2NeighborView v, int ncell
     int a[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-      a[k] = (idx + k < ncell) ? v.cell_count[idx + k] : 0;
+      a[k] = (idx + k < ncell) ? in(idx + k) : 0;
     const int mine = a[0] + a[1] + a[2] + a[3];
     int incl = mine;
 #pragma unroll
@@ -112,7 +113,7 @@ __global__ void __launch_bounds__(1024) k_scan_cells(B2NeighborView v, int ncell
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (idx + k < ncell)
-        v.cell_start[idx + k] = excl;
+        out[idx + k] = excl;
       excl += a[k];
     }
     __syncthreads();
@@ -121,7 +122,14 @@ __global__ void __launch_bounds__(1024) k_scan_cells(B2NeighborView v, int ncell
     __syncthreads();
   }
   if (tid == 0)
-    v.cell_start[ncell] = carry_s;
+    out[ncell] = carry_s;
+}
+
+__global__ void __launch_bounds__(1024) k_scan_cells(B2NeighborView v, int ncell)
+{
+  if (!v.flags[0])
+    return;
+  block_scan_1024(ncell, v.cell_start, [&](int c) { return v.cell_count[c]; });
 }
 
 __global__ void __launch_bounds__(BLK) k_cell_fill(B2NeighborView v)
@@ -283,6 +291,23 @@ __global__ void __launch_bounds__(BLK) k_tile_fill(B2NeighborView v)
   }
 }
 
+// ---- warp schedule (b2_neighbor.cuh): segments per brick -> first position of each brick -> order ----
+__global__ void __launch_bounds__(1024) k_brick_scan(B2NeighborView v, B2Grid g, B2Bricks br)
+{
+  if (!v.flags[0])
+    return;
+  block_scan_1024(br.count, v.brick_start, [&](int b) { return b2_body_brick_count(b, v, g, br); });
+}
+
+__global__ void __launch_bounds__(BLK) k_seg_order(B2NeighborView v, B2Grid g, B2Bricks br)
+{
+  if (!v.flags[0])
+    return;
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < br.count)
+    b2_body_seg_order(b, v, g, br);
+}
+
 __global__ void k_rebuild_done(int* flags)
 {
   if (flags[0]) {
@@ -363,6 +388,8 @@ B2NeighborView Neighbor::view() const
   v.tile_type = tile_type.p;
   v.tile_blk = tile_blk.p;
   v.tile_meta = tile_meta.p;
+  v.seg_order = schedule ? seg_order.p : nullptr;
+  v.brick_start = brick_start.p;
   return v;
 }
 
@@ -405,6 +432,8 @@ int Neighbor::update(
     B2_CUDA(cell_count.reserve(cap));
     B2_CUDA(cell_fill.reserve(cap));
     B2_CUDA(cell_start.reserve(cap + 1));
+    if (schedule)
+      B2_CUDA(brick_start.reserve(cap + 1)); // never more bricks than cells
   }
   if (have_grid && (g.nb[0] != grid.nb[0] || g.nb[1] != grid.nb[1] || g.nb[2] != grid.nb[2])) {
     k_force_rebuild<<<1, 1, 0, st>>>(flags.p);
@@ -449,8 +478,22 @@ int Neighbor::update(
     k_tile_fill<<<gn, BLK, 0, st>>>(v);
     B2_LAUNCHED();
   }
+  if (schedule) {
+    const B2Bricks br = b2_make_bricks(g, n);
+    k_brick_scan<<<1, 1024, 0, st>>>(v, g, br);
+    B2_LAUNCHED();
+    k_seg_order<<<grid_for(br.count, BLK), BLK, 0, st>>>(v, g, br);
+    B2_LAUNCHED();
+  }
   k_rebuild_done<<<1, 1, 0, st>>>(flags.p);
   B2_LAUNCHED();
+  return B200MD_OK;
+}
+
+int Neighbor::enable_schedule()
+{
+  B2_CUDA(seg_order.reserve(((size_t)capacity + 31) / 32));
+  schedule = true;
   return B200MD_OK;
 }
 

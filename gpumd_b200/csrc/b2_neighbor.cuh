@@ -67,7 +67,38 @@ struct B2NeighborView {
   int* tile_type = nullptr; // [tile_nslot / 128] type of each 128-slot tile
   int* tile_blk = nullptr;  // [tile_nt * tile_nblk] per-block counts, then offsets inside the bucket
   int* tile_meta = nullptr; // [0] number of tiles, [1 + t] first slot of type t
+  // optional warp schedule (Neighbor::enable_schedule): a permutation of the SEGMENTS (the 32 consecutive
+  // sorted atoms [32 s, 32 s + 32)) that puts the segments of one brick of cells next to each other, so
+  // that the warps of a block, and the blocks resident on an SM, gather from the same neighbourhood.
+  // No atom moves: a consumer maps warp w to atoms seg_order[w] * 32 + lane, and any permutation is correct
+  int* seg_order = nullptr;   // [ceil(n / 32)]
+  int* brick_start = nullptr; // [number of bricks] first position of each brick in seg_order
 };
+
+// Bricks of the schedule: bx x by x bz cells, numbered y fastest, then x, then z (consecutive blocks, which
+// run at the same time on the same or nearby SMs, are then bricks stacked along y over the same cells in x:
+// measured faster than x fastest, see DESIGN 6; z outermost keeps consecutive blocks close in memory).  by = bz = 2 rows; bx = the cells that 32
+// atoms span at the mean density, so that the four warps of a 128-thread block are the four rows of one
+// brick.
+struct B2Bricks {
+  int bx, by, bz;
+  int nx, ny, nz; // bricks per direction
+  int count;      // nx*ny*nz
+};
+
+inline B2Bricks b2_make_bricks(const B2Grid& g, int n)
+{
+  B2Bricks b;
+  const long long span = ((long long)32 * g.ncell + n / 2) / n; // cells per segment, rounded
+  b.bx = span < 1 ? 1 : (span > g.nb[0] ? g.nb[0] : (int)span);
+  b.by = 2;
+  b.bz = 2;
+  b.nx = (g.nb[0] + b.bx - 1) / b.bx;
+  b.ny = (g.nb[1] + b.by - 1) / b.by;
+  b.nz = (g.nb[2] + b.bz - 1) / b.bz;
+  b.count = b.nx * b.ny * b.nz;
+  return b;
+}
 
 // ---- pack: caller SoA -> sorted B2Atom records, and displacement trigger -------------------
 // (gpu_check_atom_distance, neighbor.cu:646-684; the trigger only needs to be conservative)
@@ -276,3 +307,41 @@ B2_HD void b2_body_skin_reverse(int i, const B2NeighborView& v)
   }
 }
 
+// ---- warp schedule ---------------------------------------------------------------------------
+// Order of the segments: by the brick (cz / bz, cx / bx, cy / by) of the cell of the segment's FIRST atom,
+// inside a brick by (cz % bz, cy % by, cx), ties by segment number.  The atoms are sorted by cell with x
+// fastest, so the segments that start in the cells [c0, c1) of one row are the consecutive numbers
+// ceil(cell_start[c0] / 32) .. ceil(cell_start[c1] / 32) - 1: the order follows from cell_start alone,
+// without a sort.  fn(s) is called for the segments of brick b in that order; returns their number.
+template <class Fn>
+B2_HD int b2_brick_segments(int b, const B2Grid& g, const B2Bricks& br, const int* cell_start, Fn fn)
+{
+  const int ky = b % br.ny, kx = (b / br.ny) % br.nx, kz = b / (br.nx * br.ny);
+  const int x0 = kx * br.bx, x1 = x0 + br.bx < g.nb[0] ? x0 + br.bx : g.nb[0];
+  int count = 0;
+  for (int rz = 0; rz < br.bz; ++rz) {
+    for (int ry = 0; ry < br.by; ++ry) {
+      const int cy = ky * br.by + ry, cz = kz * br.bz + rz;
+      if (cy >= g.nb[1] || cz >= g.nb[2])
+        continue;
+      const int row = g.nb[0] * (cy + g.nb[1] * cz);
+      const int s1 = (cell_start[row + x1] + 31) >> 5;
+      for (int s = (cell_start[row + x0] + 31) >> 5; s < s1; ++s) {
+        fn(s);
+        ++count;
+      }
+    }
+  }
+  return count;
+}
+
+B2_HD int b2_body_brick_count(int b, const B2NeighborView& v, const B2Grid& g, const B2Bricks& br)
+{
+  return b2_brick_segments(b, g, br, v.cell_start, [](int) {});
+}
+
+B2_HD void b2_body_seg_order(int b, const B2NeighborView& v, const B2Grid& g, const B2Bricks& br)
+{
+  int* out = v.seg_order + v.brick_start[b];
+  b2_brick_segments(b, g, br, v.cell_start, [&](int s) { *out++ = s; });
+}

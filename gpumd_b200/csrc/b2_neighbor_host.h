@@ -40,6 +40,8 @@ public:
   bool reverse = false;
   int tile_nt = 0; // type tiles (see B2NeighborView) are maintained when > 0
   DevBuf<int> tile_atom, tile_slot, tile_type, tile_blk, tile_meta;
+  bool schedule = false; // see B2NeighborView::seg_order (enable_schedule)
+  DevBuf<int> seg_order, brick_start;
 
   // Neighbor::initialize, src/force/neighbor.cu:824-833
   int init(int num_atoms, double rc, int mn_skin);
@@ -49,6 +51,9 @@ public:
   int enable_planes();
   // also maintain the reverse slots of the skin list (column-major, untagged lists; call after init)
   int enable_reverse();
+  // also maintain the warp schedule seg_order at every rebuild (call after init)
+  int enable_schedule();
+  int num_segments() const { return (n + 31) / 32; }
   int max_tiles() const { return (n + 127) / 128 + tile_nt; }
   // Neighbor::find_neighbor_global, src/force/neighbor.cu:756-800 (fully asynchronous here)
   int update(const B2Box& box, const int* d_type, const double* d_pos, int n, cudaStream_t st);

@@ -345,6 +345,7 @@ struct b200md_nep {
                           // than the shared-memory accumulators on UNEP-v1, B200MD_NEP_RADREG=1
   bool ang_cstage = true; // k_desc_angular: coefficient table staged in shared memory
   bool radial_v2 = false; // few-type radial passes of b2_nep_radial.cuh (planes, branch-free loop)
+  bool sched = false;     // their warps follow Neighbor::seg_order (B200MD_NEP_SCHED=0: identity, A/B runs)
   // small periodic boxes (SURVEY 8f rank 1): supercell replication, see b200md_nep_compute
   DevBuf<int> rep_type;
   DevBuf<double> rep_pos, rep_out;
@@ -390,7 +391,7 @@ int dispatch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
     B2RadialDescArgs A;
     A.n = P.n; A.nt = P.nt; A.nr1 = P.nr1; A.mn_r = P.mn_r; A.mn_a = P.mn_a;
     A.plane0 = p->nb.plane0.p; A.plane1 = p->nb.plane1.p; A.planez = p->nb.planez.p;
-    A.nn_skin = P.nn_skin; A.nl_skin = P.nl_skin;
+    A.nn_skin = P.nn_skin; A.nl_skin = P.nl_skin; A.seg_order = P.seg_order;
     A.nn_r = P.nn_r; A.nl_r = P.nl_r; A.nn_a = P.nn_a; A.nl_a = P.nl_a;
     A.q = P.q; A.flags = P.flags;
     A.tile_slot = P.tile_slot; A.qt = P.qt; A.DKT = P.DKT;
@@ -793,6 +794,12 @@ int nep_setup(b200md_nep* p, int num_atoms)
   p->use_tc = m.tc_ok && !mlp_simt && !fused_fits;
   if (p->radial_v2)
     B2_TRY(p->nb.enable_planes());
+  {
+    const char* e = std::getenv("B200MD_NEP_SCHED");
+    p->sched = p->radial_v2 && !(e && e[0] == '0');
+    if (p->sched)
+      B2_TRY(p->nb.enable_schedule());
+  }
   const int pitch_r = (m.MN_radial + 7) / 8 * 8;
   // B200MD_NEP_REVSLOT=1 (many types with the neighbour split as its own kernel): direct reverse slots
   // for the angular pair reduction instead of a binary search per pair: k_force_final gets faster on
@@ -820,7 +827,7 @@ int nep_setup(b200md_nep* p, int num_atoms)
     B2_CUDA(p->FpA.reserve(N * m.dim_angular));
   }
   B2_CUDA(p->U.reserve(N * m.UST));
-  B2_CUDA(p->f12.reserve(N * 3 * m.MN_angular));
+  B2_CUDA(p->f12.reserve(N * (p->radial_v2 ? 4 : 3) * m.MN_angular)); // few types: float4 entries
   if (p->radial_v2)
     B2_CUDA(p->arev.reserve(N * m.MN_angular));
   B2_CUDA(p->acc.reserve(N)); // site energies from the MLP pass
@@ -902,6 +909,7 @@ int nep_setup(b200md_nep* p, int num_atoms)
   P.f12 = p->f12.p;
   P.acc = p->acc.p;
   P.flags = p->nb.flags.p;
+  P.seg_order = p->sched ? p->nb.seg_order.p : nullptr;
   P.team = team ? 1 : 0;
   P.u_planes = p->radial_v2 ? 2 : (team ? 1 : 0);
   P.pitch_r = pitch_r;
@@ -1024,6 +1032,7 @@ int b200md_nep_info(const b200md_nep* p, int what)
       const_cast<b200md_nep*>(p)->nb.check(0, &bits, &rebuilds);
       return rebuilds;
     }
+    case 7: return p->sched ? p->nb.num_segments() : 0;
     default: return -1;
   }
 }
@@ -1195,6 +1204,30 @@ int b200md_nep_export_descriptors(b200md_nep* p, float* d_q, void* stream)
   k_export_q<<<grid_for(p->n, 128), 128, 0, (cudaStream_t)stream>>>(
     p->view, p->rep_n ? p->rep_n : p->n, d_q);
   B2_LAUNCHED();
+  return B200MD_OK;
+}
+
+int b200md_nep_export_schedule(
+  b200md_nep* p, int dims[6], int* d_seg_order, int* d_cell_start, void* stream)
+{
+  if (!p->sched || !p->nb.have_grid) {
+    set_error("b200md_nep_export_schedule: no schedule (identity schedule, or no compute call yet)");
+    return B200MD_ERR_ARG;
+  }
+  const B2Grid& g = p->nb.grid;
+  const B2Bricks br = b2_make_bricks(g, p->nb.n);
+  for (int d = 0; d < 3; ++d)
+    dims[d] = g.nb[d];
+  dims[3] = br.bx;
+  dims[4] = br.by;
+  dims[5] = br.bz;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d_seg_order)
+    B2_CUDA(cudaMemcpyAsync(d_seg_order, p->nb.seg_order.p, sizeof(int) * p->nb.num_segments(),
+                            cudaMemcpyDeviceToDevice, st));
+  if (d_cell_start)
+    B2_CUDA(cudaMemcpyAsync(d_cell_start, p->nb.cell_start.p, sizeof(int) * ((size_t)g.ncell + 1),
+                            cudaMemcpyDeviceToDevice, st));
   return B200MD_OK;
 }
 

@@ -111,7 +111,7 @@ struct B2NepView {
   float* FpR; // [nr1 * n]     dU/dq, radial part (input of k_utable)
   float* FpA; // [dim_ang * n] dU/dq (already multiplied by q_scaler), angular part
   float* U;   // [n * UST]   pre-contracted radial table
-  float* f12; // [3 * mn_a * n]
+  float* f12; // [3 * mn_a * n] as three planes; few-type kernels: [mn_a * n] float4 entries (w unused)
   double* acc; // [13 * n]: pe, fx,fy,fz, virial xx,yy,zz,xy,xz,yz,yx,zx,zy (sorted order)
   int* flags;
   // ---- lane-team path (<= 2 types): row-major skin / radial lists, U table as float4 planes ----
@@ -144,6 +144,7 @@ struct B2NepView {
   const int* tile_atom; // B2NeighborView::tile_atom / tile_type / tile_meta
   const int* tile_type;
   const int* tile_meta;
+  const int* seg_order; // B2NeighborView::seg_order (few-type kernels); null = identity schedule
 };
 
 // address of descriptor component k of sorted atom i (slot = P.tile_slot[i] when the tile-major copy is

@@ -207,7 +207,7 @@ __device__ __forceinline__ void b2_ang_force_pairs(
   const int* __restrict__ list = P.nl_a;
   const int* __restrict__ cnt = P.nn_a;
   const int nn = cnt[i];
-  const size_t plane = (size_t)P.mn_a * N; // 3 planes may exceed 2^32 entries
+  float4* __restrict__ f4 = reinterpret_cast<float4*>(P.f12);
   // list entries two neighbours ahead; position and list length of the neighbour one ahead
   int e1 = nn > 1 ? __ldg(list + N + i) : i;
   int en = nn > 0 ? __ldg(list + i) : i;
@@ -300,9 +300,7 @@ __device__ __forceinline__ void b2_ang_force_pairs(
     b2_harmonics_grad_dot(xh, yh, zh, W, gx, gy, gz);
     const float rad = ar - al * dinv;
     const unsigned slot = (unsigned)m * N + i;
-    P.f12[slot] = fmaf(rad, xh, gx * dinv);
-    P.f12[plane + slot] = fmaf(rad, yh, gy * dinv);
-    P.f12[2 * plane + slot] = fmaf(rad, zh, gz * dinv);
+    f4[slot] = make_float4(fmaf(rad, xh, gx * dinv), fmaf(rad, yh, gy * dinv), fmaf(rad, zh, gz * dinv), 0.0f);
     arev[slot] = hit ? below : 0;
   }
 }

@@ -182,6 +182,22 @@ class NEP(Potential):
         self.check()
         return NNr.cpu().numpy(), NLr.cpu().numpy(), NNa.cpu().numpy(), NLa.cpu().numpy()
 
+    def export_schedule(self):
+        """The warp schedule of the last list rebuild: dict(nb, brick, seg_order, cell_start), or None
+        when the handle runs the identity schedule."""
+        nseg = self._L.b200md_nep_info(self._h, 7)
+        if nseg == 0:
+            return None
+        dims = (C.c_int * 6)()
+        _lib.check(self._L.b200md_nep_export_schedule(self._h, dims, None, None, _stream()))
+        nb = [int(x) for x in dims[:3]]
+        order = torch.zeros(nseg, dtype=torch.int32, device="cuda")
+        start = torch.zeros(nb[0] * nb[1] * nb[2] + 1, dtype=torch.int32, device="cuda")
+        _lib.check(self._L.b200md_nep_export_schedule(self._h, dims, _ptr(order), _ptr(start), _stream()))
+        self.check()
+        return dict(nb=nb, brick=[int(x) for x in dims[3:]], seg_order=order.cpu().numpy(),
+                    cell_start=start.cpu().numpy())
+
     def export_descriptors(self):
         q = torch.zeros(self.dim, self.N2, dtype=torch.float32, device="cuda")
         _lib.check(self._L.b200md_nep_export_descriptors(self._h, _ptr(q), _stream()))

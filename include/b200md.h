@@ -49,7 +49,8 @@ int b200md_nep_create(const char* nep_txt_path, int num_atoms, b200md_nep** out)
 void b200md_nep_destroy(b200md_nep* p);
 
 /* what: 0 num_types, 1 descriptor dim, 2 neurons, 3 MN_radial (enlarged), 4 MN_angular
- * (enlarged), 5 zbl enabled, 6 number of neighbour-list rebuilds so far */
+ * (enlarged), 5 zbl enabled, 6 number of neighbour-list rebuilds so far, 7 segments of the warp
+ * schedule (0: identity schedule, see b200md_nep_export_schedule) */
 int b200md_nep_info(const b200md_nep* p, int what);
 double b200md_nep_rc(const b200md_nep* p); /* Potential::rc, src/force/potential.cuh:32 */
 /* atomic symbol of type t (species -> type index mapping, src/model/read_xyz.cu:349-361) */
@@ -77,6 +78,14 @@ int b200md_nep_export_neighbors(
 int b200md_transpose_int(int n, int mn, const int* d_row_major, int* d_column_major, void* stream);
 /* Parity hook: scaled descriptors q[d*N + i] (caller order) of the last compute call. */
 int b200md_nep_export_descriptors(b200md_nep* p, float* d_q, void* stream);
+
+/* Parity hook: the warp schedule of the one- and two-species kernels as of the last list rebuild.  A segment
+ * is 32 consecutive cell-sorted atoms; warp w evaluates segment seg_order[w].  dims = cells per direction
+ * (3), cells per brick (3); d_seg_order[b200md_nep_info(p, 7)] and d_cell_start[cells + 1] (first sorted
+ * atom of every cell, x fastest) are device pointers, each may be null.  Error when the handle runs the
+ * identity schedule (B200MD_NEP_SCHED=0, or a model with more than two species). */
+int b200md_nep_export_schedule(
+  b200md_nep* p, int dims[6], int* d_seg_order, int* d_cell_start, void* stream);
 
 /* synchronise and report latched device-side errors (B200MD_ERR_OVERFLOW) */
 int b200md_nep_check(b200md_nep* p, void* stream);
