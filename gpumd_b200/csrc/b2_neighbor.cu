@@ -341,6 +341,7 @@ int Neighbor::init(int num_atoms, double rc_, int mn_skin_)
   B2_CUDA(atoms.reserve(n));
   B2_CUDA(atoms_tmp.reserve(n));
   B2_CUDA(snap.reserve((size_t)3 * n));
+  B2_CUDA(snap_type.reserve(n));
   B2_CUDA(perm.reserve(n));
   B2_CUDA(perm_tmp.reserve(n));
   B2_CUDA(cell_of.reserve(n));
@@ -349,6 +350,7 @@ int Neighbor::init(int num_atoms, double rc_, int mn_skin_)
   B2_CUDA(nl_skin.reserve((size_t)skin_pitch() * n));
   B2_CUDA(flags.reserve(4));
   B2_CUDA(cudaMemset(snap.p, 0, sizeof(double) * 3 * (size_t)n));
+  B2_CUDA(cudaMemset(snap_type.p, 0, sizeof(int) * (size_t)n));
   k_init_perm<<<grid_for(n, BLK), BLK>>>(n, perm.p, flags.p);
   B2_LAUNCHED();
   have_grid = false;
@@ -368,6 +370,7 @@ B2NeighborView Neighbor::view() const
   v.tag_types = tag_types ? 1 : 0;
   v.rskin = reverse ? rskin.p : nullptr;
   v.snap = snap.p;
+  v.snap_type = snap_type.p;
   v.perm = perm.p;
   v.perm_tmp = perm_tmp.p;
   v.cell_of = cell_of.p;

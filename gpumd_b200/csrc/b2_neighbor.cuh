@@ -36,11 +36,16 @@ struct B2NeighborView {
   int4* plane1 = nullptr;
   double* planez = nullptr; // z alone (8 bytes, 16 atoms per line) for consumers that get the type elsewhere
   // 1: skin-list entries carry the neighbour's type in bits 30+ (entry = j | type << 30; needs
-  //    n < 2^30 and <= 2 types).  The type of an atom is constant between rebuilds, and a consumer that
-  //    reads it from the entry saves a gather.  Only the few-type NEP kernels ask for this.
+  //    n < 2^30 and <= 2 types).  The type of an atom is constant between rebuilds (a changed type
+  //    rebuilds, b2_body_pack_check), and a consumer that reads it from the entry saves a gather.  Only
+  //    the few-type NEP kernels ask for this.
   int tag_types = 0;
   double* snap;      // [3n] positions at the last rebuild, sorted order (x0,y0,z0 SoA)
-  int* perm;         // [n] sorted index -> caller index
+  // [n] types at the last rebuild, sorted order: a changed type rebuilds, because the type tags of the skin
+  // list and the type tiles are built from them.  Neighbor always keeps it; null (a view built without the
+  // snapshot) = only displacements rebuild
+  int* snap_type = nullptr;
+  int* perm;        // [n] sorted index -> caller index
   int* perm_tmp;     // [n]
   int* cell_of;      // [n] cell id of sorted atom (valid during a rebuild)
   int* order_tmp;    // [n] old sorted index per new slot
@@ -143,7 +148,8 @@ B2_HD void b2_body_pack_check(
   float dy = (float)(a.y - v.snap[(size_t)v.n + i]);
   float dz = (float)(a.z - v.snap[(size_t)2 * v.n + i]);
   b2_mic(box, dx, dy, dz);
-  if (dx * dx + dy * dy + dz * dz > trigger_d2)
+  // a swapped or changed species (Monte Carlo moves between MD steps) rebuilds like a displacement
+  if (dx * dx + dy * dy + dz * dz > trigger_d2 || (v.snap_type && a.type != v.snap_type[i]))
     v.flags[0] = 1; // benign race: every writer stores the same value
 }
 
@@ -206,6 +212,8 @@ B2_HD void b2_body_commit(int i, const B2NeighborView& v)
   v.snap[i] = a.x;
   v.snap[(size_t)v.n + i] = a.y;
   v.snap[(size_t)2 * v.n + i] = a.z;
+  if (v.snap_type)
+    v.snap_type[i] = a.type;
 }
 
 // Offsets -2..+2 of one direction arranged so that the WRAPPED coordinate ascends.

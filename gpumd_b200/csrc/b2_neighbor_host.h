@@ -34,7 +34,7 @@ public:
   bool planes = false;
   bool tag_types = false; // see B2NeighborView::tag_types (set before the first update)
   DevBuf<double> snap;
-  DevBuf<int> perm, perm_tmp, cell_of, order_tmp, cell_count, cell_fill, cell_start, nn_skin,
+  DevBuf<int> snap_type, perm, perm_tmp, cell_of, order_tmp, cell_count, cell_fill, cell_start, nn_skin,
     nl_skin, flags;
   DevBuf<int> rskin;    // see B2NeighborView::rskin (enable_reverse)
   bool reverse = false;

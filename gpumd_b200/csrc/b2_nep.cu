@@ -266,6 +266,55 @@ __global__ void k_export_q(B2NepView P, int n_cell, float* out)
     out[(size_t)d * n_cell + a] = *b2_q_ptr(P, i, P.qt ? P.tile_slot[i] : 0, d) * P.q_scaler[d];
 }
 
+__global__ void k_export_tile_slot(int n, int n_cell, const int* perm, const int* tile_slot, int* out)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const int a = perm[i];
+  if (a < n_cell)
+    out[a] = tile_slot[i];
+}
+
+// the hidden layer's output in one layout whatever the storage: fp[d*n_cell + a] (dU/dq times q_scaler)
+// and u[(t2*K1R + k)*n_cell + a] (the U table); either may be null
+__global__ void k_export_mlp(B2NepView P, int n_cell, float* fp, float* u)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P.n)
+    return;
+  const int a = P.perm[i];
+  if (a >= n_cell)
+    return;
+  const size_t N = (size_t)P.n, M = (size_t)n_cell;
+  if (fp) {
+    for (int d = 0; d < P.dim; ++d) {
+      float v;
+      if (P.fpt)
+        v = P.fpt[b2_tile_offset(P.DKT, P.tile_slot[i], d)];
+      else
+        v = d < P.nr1 ? P.FpR[(size_t)d * N + i] : P.FpA[(size_t)(d - P.nr1) * N + i];
+      fp[(size_t)d * M + a] = v;
+    }
+  }
+  if (u) {
+    const int KQ = P.KP / 4 - 1;
+    for (int t2 = 0; t2 < P.nt; ++t2) {
+      for (int k = 0; k < P.K1R; ++k) {
+        float v;
+        if (P.u_planes == 2) // compact planes (b2_nep_radial.cuh): k < K1R - 1 in float4 planes, the last alone
+          v = k < 4 * KQ ? P.U[((size_t)(t2 * KQ + k / 4) * N + i) * 4 + (k & 3)]
+                         : P.U[(size_t)P.nt * KQ * 4 * N + (size_t)t2 * N + i];
+        else if (P.u_planes == 1) // float4 planes [(t2*KP4 + q)*n + i]
+          v = P.U[((size_t)((t2 * P.KP + k) / 4) * N + i) * 4 + (k & 3)];
+        else // AoS rows of UST floats
+          v = P.U[(size_t)i * P.UST + t2 * P.KP + k];
+        u[((size_t)t2 * P.K1R + k) * M + a] = v;
+      }
+    }
+  }
+}
+
 // ---- small periodic boxes: evaluate a supercell, keep the first replica -----------------------
 // replica r = (a*ry + b)*rz + c of atom i sits at index r*n + i, shifted by a*A + b*B + c*C
 __global__ void __launch_bounds__(BLK) k_replicate(
@@ -333,7 +382,9 @@ struct b200md_nep {
   DevBuf<double> acc;
   DevBuf<float> tc_img, qt, fpt; // tile-major q / dU/dq for k_mlp_tc (B2NepView::qt)
   int num_sms = 132;
-  int variant = 0;         // B200MD_NEP_VARIANT: kernel tuning variants for A/B measurements
+  int tc_ctas_cap = 0;  // B200MD_NEP_TC_CTAS: at most this many CTAs of k_mlp_tc (0: as many as fit)
+  int tc_ctas_last = 0; // CTAs of the last k_mlp_tc launch (0: the last compute did not run it)
+  int variant = 0;        // B200MD_NEP_VARIANT: kernel tuning variants for A/B measurements
   bool fuse_split = false; // many-type path: neighbour split inside the radial descriptor pass
   bool use_tc = false; // hidden layer on the tensor cores (k_mlp_tc) instead of k_mlp
   bool ang_fused = false; // k_angular_fused instead of k_desc_angular2 + hidden layer + k_force_angular2
@@ -663,7 +714,10 @@ int angular_stages(b200md_nep* p, const B2Box& box, cudaStream_t st)
     B2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_mlp_tc, 128, bytes));
     per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
     const int tiles = p->nb.max_tiles();
-    const int ctas = tiles < p->num_sms * per_sm ? tiles : p->num_sms * per_sm;
+    int ctas = tiles < p->num_sms * per_sm ? tiles : p->num_sms * per_sm;
+    if (p->tc_ctas_cap > 0 && ctas > p->tc_ctas_cap)
+      ctas = p->tc_ctas_cap; // every tile is still computed by one CTA with the same arithmetic
+    p->tc_ctas_last = ctas;
     k_mlp_tc<<<ctas, 128, bytes, st>>>(p->view);
     B2_LAUNCHED();
   } else
@@ -700,6 +754,7 @@ int nep_pipeline(
   b200md_nep* p, const B2Box& box, cudaStream_t st, double* d_pe, double* d_force, double* d_virial)
 {
   StageProfiler& pf = p->prof;
+  p->tc_ctas_last = 0;
   pf.begin(st, ST_DESC_R);
   switch (p->model.K1R) {
     case 9: B2_TRY(dispatch_desc_radial<9>(p, box, st)); break;
@@ -922,6 +977,9 @@ int nep_setup(b200md_nep* p, int num_atoms)
     int dev = 0;
     B2_CUDA(cudaGetDevice(&dev));
     B2_CUDA(cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, dev));
+    // B200MD_NEP_TC_CTAS=k (tests): cap the persistent CTAs so that each walks many tiles
+    if (const char* e = std::getenv("B200MD_NEP_TC_CTAS"))
+      p->tc_ctas_cap = std::atoi(e) > 0 ? std::atoi(e) : 0;
     B2_TRY(p->nb.enable_type_tiles(m.nt));
     B2_TRY(upload(p->tc_img, m.tc_img));
     P.tc_img = p->tc_img.p;
@@ -980,6 +1038,18 @@ int nep_setup(b200md_nep* p, int num_atoms)
   return B200MD_OK;
 }
 
+// type tiles of the last list rebuild (synchronises; 0 without tiles)
+int nep_tile_count(const b200md_nep* p)
+{
+  if (!p->use_tc || !p->nb.have_grid)
+    return 0;
+  int ntile = 0;
+  if (cudaDeviceSynchronize() != cudaSuccess ||
+      cudaMemcpy(&ntile, p->nb.tile_meta.p, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return -1;
+  return ntile;
+}
+
 } // namespace
 
 extern "C" {
@@ -1033,6 +1103,8 @@ int b200md_nep_info(const b200md_nep* p, int what)
       return rebuilds;
     }
     case 7: return p->sched ? p->nb.num_segments() : 0;
+    case 8: return nep_tile_count(p);
+    case 9: return p->tc_ctas_last;
     default: return -1;
   }
 }
@@ -1228,6 +1300,36 @@ int b200md_nep_export_schedule(
   if (d_cell_start)
     B2_CUDA(cudaMemcpyAsync(d_cell_start, p->nb.cell_start.p, sizeof(int) * ((size_t)g.ncell + 1),
                             cudaMemcpyDeviceToDevice, st));
+  return B200MD_OK;
+}
+
+int b200md_nep_export_tiles(b200md_nep* p, int* d_slot, int* d_tile_type, void* stream)
+{
+  const int ntile = nep_tile_count(p);
+  if (ntile <= 0) {
+    set_error("b200md_nep_export_tiles: no type tiles (SIMT hidden layer, or no compute call yet)");
+    return B200MD_ERR_ARG;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d_slot) {
+    k_export_tile_slot<<<grid_for(p->n, 128), 128, 0, st>>>(
+      p->n, p->rep_n ? p->rep_n : p->n, p->nb.perm.p, p->nb.tile_slot.p, d_slot);
+    B2_LAUNCHED();
+  }
+  if (d_tile_type)
+    B2_CUDA(cudaMemcpyAsync(d_tile_type, p->nb.tile_type.p, sizeof(int) * ntile, cudaMemcpyDeviceToDevice, st));
+  return B200MD_OK;
+}
+
+int b200md_nep_export_mlp(b200md_nep* p, float* d_fp, float* d_u, void* stream)
+{
+  if (p->ang_fused) {
+    set_error("b200md_nep_export_mlp: k_angular_fused keeps dU/dq and the U table on chip");
+    return B200MD_ERR_ARG;
+  }
+  k_export_mlp<<<grid_for(p->n, 128), 128, 0, (cudaStream_t)stream>>>(
+    p->view, p->rep_n ? p->rep_n : p->n, d_fp, d_u);
+  B2_LAUNCHED();
   return B200MD_OK;
 }
 

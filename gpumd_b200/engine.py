@@ -95,6 +95,7 @@ class NEP(Potential):
         h = C.c_void_p()
         _lib.check(self._L.b200md_nep_create(str(file_potential).encode(), int(num_atoms), C.byref(h)))
         self._h = h
+        self._path = str(file_potential)
         self.N1, self.N2 = 0, int(num_atoms)
         self.rc = self._L.b200md_nep_rc(h)
         self.num_types = self._L.b200md_nep_info(h, 0)
@@ -202,6 +203,44 @@ class NEP(Potential):
         q = torch.zeros(self.dim, self.N2, dtype=torch.float32, device="cuda")
         _lib.check(self._L.b200md_nep_export_descriptors(self._h, _ptr(q), _stream()))
         return q.cpu().numpy()
+
+    @property
+    def num_tiles(self):
+        """Type tiles of the last list rebuild (0: the SIMT hidden layer has none)."""
+        return self._L.b200md_nep_info(self._h, 8)
+
+    @property
+    def tc_ctas(self):
+        """CTAs of the last tensor-core hidden-layer launch (0: the last compute did not run it)."""
+        return self._L.b200md_nep_info(self._h, 9)
+
+    def export_tiles(self, n=None):
+        """(slot[n] of every caller-order atom, tile_type[num_tiles]) of the last list rebuild."""
+        n = n or self.N2
+        slot = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+        tile_type = torch.full((max(self.num_tiles, 1),), -1, dtype=torch.int32, device="cuda")
+        _lib.check(self._L.b200md_nep_export_tiles(self._h, _ptr(slot), _ptr(tile_type), _stream()))
+        self.check()
+        return slot.cpu().numpy(), tile_type[:self.num_tiles].cpu().numpy()
+
+    def export_mlp(self, n=None):
+        """(dU/dq [dim, n] times q_scaler, U table [num_types, K, n]) of the last compute, caller order;
+        K = the padded radial basis (9, 13 or 17)."""
+        n = n or self.N2
+        k1 = next(k for k in (9, 13, 17) if k >= self._basis_radial())
+        fp = torch.full((self.dim, n), float("nan"), dtype=torch.float32, device="cuda")
+        u = torch.full((self.num_types, k1, n), float("nan"), dtype=torch.float32, device="cuda")
+        _lib.check(self._L.b200md_nep_export_mlp(self._h, _ptr(fp), _ptr(u), _stream()))
+        self.check()
+        return fp.cpu().numpy(), u.cpu().numpy()
+
+    def _basis_radial(self):
+        with open(self._path) as f:
+            for line in f:
+                tok = line.split()
+                if tok and tok[0] == "basis_size":
+                    return int(tok[1]) + 1
+        raise _lib.B200mdError("no basis_size line in " + str(self._path))
 
 
 class LJ(Potential):

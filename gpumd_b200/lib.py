@@ -31,6 +31,8 @@ SIGNATURES = {
     "b200md_transpose_int": (C.c_int, [C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200md_nep_export_descriptors": (C.c_int, [_vp, _vp, _vp]),
     "b200md_nep_export_schedule": (C.c_int, [_vp, _ip, _vp, _vp, _vp]),
+    "b200md_nep_export_tiles": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "b200md_nep_export_mlp": (C.c_int, [_vp, _vp, _vp, _vp]),
     "b200md_nep_check": (C.c_int, [_vp, _vp]),
     "b200md_nep_profile": (C.c_int, [_vp, C.c_int]),
     "b200md_nep_profile_read": (C.c_int, [_vp, C.c_int, C.POINTER(C.c_float), _ip]),

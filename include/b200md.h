@@ -50,7 +50,9 @@ void b200md_nep_destroy(b200md_nep* p);
 
 /* what: 0 num_types, 1 descriptor dim, 2 neurons, 3 MN_radial (enlarged), 4 MN_angular
  * (enlarged), 5 zbl enabled, 6 number of neighbour-list rebuilds so far, 7 segments of the warp
- * schedule (0: identity schedule, see b200md_nep_export_schedule) */
+ * schedule (0: identity schedule, see b200md_nep_export_schedule), 8 type tiles of the last list rebuild
+ * (0: no tiles, the SIMT hidden layer), 9 CTAs of the last launch of the tensor-core hidden layer (0: the
+ * last compute did not run it).  6 and 8 synchronise the device. */
 int b200md_nep_info(const b200md_nep* p, int what);
 double b200md_nep_rc(const b200md_nep* p); /* Potential::rc, src/force/potential.cuh:32 */
 /* atomic symbol of type t (species -> type index mapping, src/model/read_xyz.cu:349-361) */
@@ -86,6 +88,18 @@ int b200md_nep_export_descriptors(b200md_nep* p, float* d_q, void* stream);
  * identity schedule (B200MD_NEP_SCHED=0, or a model with more than two species). */
 int b200md_nep_export_schedule(
   b200md_nep* p, int dims[6], int* d_seg_order, int* d_cell_start, void* stream);
+
+/* Parity hook: the type tiles of the tensor-core hidden layer as of the last list rebuild.  Atoms are
+ * bucketed by species in ascending order, each bucket padded to a multiple of 128 slots; d_slot[n] gets the
+ * slot of every caller-order atom (tile = slot / 128), d_tile_type[b200md_nep_info(p, 8)] the species of
+ * every tile.  Device pointers, each may be null.  Error when the handle has no tiles. */
+int b200md_nep_export_tiles(b200md_nep* p, int* d_slot, int* d_tile_type, void* stream);
+/* Parity hook: the hidden layer's output of the last compute call, in caller order whatever the storage:
+ * d_fp[d*n + i] = dU/dq_d times q_scaler[d] (as the force kernels read it, d < descriptor dim) and
+ * d_u[(t2*K + k)*n + i] = sum_m dU/dq_m c_radial(t_i, t2, m, k), the radial U table (K = basis_size_radial + 1
+ * padded to 9, 13 or 17; zero beyond the model's basis).  Device pointers, each may be null.  Error on the
+ * fused one- and two-species kernel, where neither reaches memory. */
+int b200md_nep_export_mlp(b200md_nep* p, float* d_fp, float* d_u, void* stream);
 
 /* synchronise and report latched device-side errors (B200MD_ERR_OVERFLOW) */
 int b200md_nep_check(b200md_nep* p, void* stream);

@@ -63,7 +63,7 @@ struct EmuNeighbor {
   double rc = 0, skin = 1.0;
   std::vector<B2Atom> atoms, atoms_tmp;
   std::vector<double> snap;
-  std::vector<int> perm, perm_tmp, cell_of, order_tmp, cell_count, cell_fill, cell_start, nn_skin,
+  std::vector<int> snap_type, perm, perm_tmp, cell_of, order_tmp, cell_count, cell_fill, cell_start, nn_skin,
     nl_skin, flags, rskin;
   bool reverse = false; // mirrors Neighbor::enable_reverse
   B2NeighborView v;
@@ -79,6 +79,7 @@ struct EmuNeighbor {
     atoms.resize(n);
     atoms_tmp.resize(n);
     snap.assign((size_t)3 * n, 0.0);
+    snap_type.assign(n, 0);
     perm.resize(n);
     for (int i = 0; i < n; ++i)
       perm[i] = i;
@@ -112,6 +113,7 @@ struct EmuNeighbor {
     v.atoms = atoms.data();
     v.atoms_tmp = atoms_tmp.data();
     v.snap = snap.data();
+    v.snap_type = snap_type.data();
     v.perm = perm.data();
     v.perm_tmp = perm_tmp.data();
     v.cell_of = cell_of.data();

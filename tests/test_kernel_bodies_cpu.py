@@ -182,6 +182,31 @@ def test_skin_list_reuse_and_rebuild(oracle, emu):
         assert_close(out["force"], r["force"], **TOL["force"], what="force")
 
 
+def test_changed_types_rebuild(oracle, emu):
+    """Same positions, 5 % of the unlike pairs swapped: exactly one rebuild (a changed type triggers it like a
+    displacement), none when the same types come again; the result equals a fresh handle's bit for bit and
+    the oracle's."""
+    s = rocksalt_pbte(4, rattle=0.05, seed=1)
+    n = s["type"].shape[0]
+    t2 = s["type"].copy()
+    rng = np.random.default_rng(5)
+    pb, te = rng.permutation(np.nonzero(t2 == 0)[0])[:13], rng.permutation(np.nonzero(t2 == 1)[0])[:13]
+    t2[pb], t2[te] = 1, 0
+    dev = emu.nep(GOLDEN / "nep_PbTe.txt", n)
+    dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
+    assert dev.rebuilds == 1
+    rc, out = dev.compute(t2, s["h"], s["pbc"], s["pos"])
+    assert rc == 0 and dev.rebuilds == 2
+    _, fresh = emu.nep(GOLDEN / "nep_PbTe.txt", n).compute(t2, s["h"], s["pbc"], s["pos"])
+    for k in ("pe", "force", "virial"):
+        assert np.array_equal(out[k], fresh[k]), k
+    dev.compute(t2, s["h"], s["pbc"], s["pos"])
+    assert dev.rebuilds == 2
+    r = oracle.NepOracle(GOLDEN / "nep_PbTe.txt").compute(t2, s["h"], s["pbc"], s["pos"], precision=32)
+    assert_close(out["force"], r["force"], **TOL["force"], what="force")
+    assert abs(out["pe"].sum() - r["pe"].sum()) / n < TOL["energy_per_atom"]
+
+
 def test_cutoff_boundary_membership(oracle, emu):
     """Pairs placed within a few ulps of the radial and angular cutoffs: membership is decided by
     the reference's FP32 expression, so the CUDA-side test and the oracle must agree exactly."""
