@@ -1015,5 +1015,128 @@ class Compute:
         return None
 
 
+# record indices of b200md_minimizer_* (include/b200md.h)
+MIN_FMAX, MIN_U, MIN_CONVERGED, MIN_DT, MIN_ALPHA, MIN_NNEG, MIN_P, MIN_FMOD, MIN_VMOD, MIN_UPHILL = range(10)
+MIN_PRESSURE, MIN_STRESS, MIN_STEP, MIN_UTRIAL, MIN_USMALLER, MIN_SCALE, MIN_LSCALE = range(10, 17)
+MIN_DEPS, MIN_VBOX, MIN_FBOX, MIN_RECORD = 17, 26, 35, 44
+SD_MIN_STEP = 1e-8  # minimizer_sd.cu:25
+
+
+class Minimizer:
+    """`minimize sd|fire tol steps [box_change [hydrostatic]]`, src/minimize/minimize.cu:32-156.
+    method 'sd' or 'fire'.  compute(force, box, atom, label, fixed_group) runs the whole minimization as
+    Minimizer::compute does (the force evaluations through `force`, everything else on the device) and
+    returns the reference's progress lines and the record of every iteration.  SD honours the fixed group
+    (label: device int tensor of the grouping method's labels); FIRE ignores it, as the reference.  With
+    box change box.cpu_h is updated in place."""
+
+    def __init__(self, method, num_atoms, force_tolerance, number_of_steps, box_change=0, hydrostatic=0):
+        _require_cuda()
+        self._L = _lib.load()
+        self.method = {"sd": 0, "fire": 1}[method]
+        self.n = int(num_atoms)
+        self.tol = float(force_tolerance)
+        self.steps = int(number_of_steps)
+        self.box_change, self.hydrostatic = int(box_change), int(hydrostatic)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_minimizer_create(self.method, self.n, self.tol, self.steps, self.box_change,
+                                                   self.hydrostatic, C.byref(h)))
+        self._h = h
+        self._rec = np.zeros(MIN_RECORD)
+        if self.method == 0:  # the reference's _temp vectors (minimizer.cuh:38-40)
+            z = dict(dtype=torch.float64, device="cuda")
+            self.trial_position, self.trial_force = torch.zeros(3 * self.n, **z), torch.zeros(3 * self.n, **z)
+            self.trial_potential = torch.zeros(self.n, **z)
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.b200md_minimizer_destroy(self._h)
+            self._h = None
+
+    @property
+    def _r(self):
+        return self._rec.ctypes.data_as(C.POINTER(C.c_double))
+
+    def velocity_ptr(self):
+        return self._L.b200md_minimizer_velocity(self._h)
+
+    def set_record(self, rec):
+        self._rec[:] = rec
+        _lib.check(self._L.b200md_minimizer_set_record(self._h, self._r, _stream()))
+
+    def fire_step(self, box, atom):
+        """One FIRE iteration after the force evaluation; returns the record."""
+        _lib.check(self._L.b200md_minimizer_fire_step(
+            self._h, self.n, box._h, _ptr(atom.position_per_atom), _ptr(atom.force_per_atom),
+            _ptr(atom.potential_per_atom), _ptr(atom.virial_per_atom), self._r, _stream()))
+        return self._rec.copy()
+
+    def _sd(self, fn, atom, label, fixed_group):
+        lab = None if label is None else _ptr(label)
+        _lib.check(fn(self._h, self.n, _ptr(atom.position_per_atom), _ptr(atom.force_per_atom),
+                      _ptr(atom.potential_per_atom), _ptr(self.trial_position), _ptr(self.trial_force),
+                      _ptr(self.trial_potential), lab, int(fixed_group), self._r, _stream()))
+        return self._rec.copy()
+
+    def sd_begin(self, atom, label=None, fixed_group=-1):
+        return self._sd(self._L.b200md_minimizer_sd_begin, atom, label, fixed_group)
+
+    def sd_step(self, atom, label=None, fixed_group=-1):
+        return self._sd(self._L.b200md_minimizer_sd_step, atom, label, fixed_group)
+
+    def compute(self, force, box, atom, label=None, fixed_group=-1):
+        base = self.steps // 10 if self.steps >= 10 else 1
+        lines, records = [], []
+        a = atom
+        if self.method == 0:  # minimizer_sd.cu:70-169
+            force.compute(box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
+                          a.virial_per_atom)
+            rec = self.sd_begin(a, label, fixed_group)
+            for step in range(self.steps):
+                if rec[MIN_CONVERGED]:
+                    lines.append("    step %d: f_max = %g eV/A." % (step, rec[MIN_FMAX]))
+                    break
+                force_max = rec[MIN_FMAX]
+                # the virial of the trial evaluation overwrites the caller's, as in the reference
+                force.compute(box, self.trial_position, a.type, self.trial_potential, self.trial_force,
+                              a.virial_per_atom)
+                rec = self.sd_step(a, label, fixed_group)
+                records.append(rec)
+                u = rec[MIN_USMALLER]
+                if rec[MIN_STEP] < SD_MIN_STEP:
+                    lines.append("    step %d: total_potential = %.10f eV, f_max = %.10f eV/A." % (
+                        step + 1, u, force_max))
+                    lines.append("    Position step is 0, SD minimizer can't find a better solution")
+                    break
+                if step == 0:
+                    lines.append("    step 0: total_potential = %.10f eV, f_max = %.10f eV/A." % (u, force_max))
+                if (step + 1) % base == 0:
+                    lines.append("    step %d: total_potential = %.10f eV, f_max = %.10f eV/A." % (
+                        step + 1, u, force_max))
+            return lines, records
+        for step in range(self.steps):  # minimizer_fire.cu:108-180, minimizer_fire_box_change.cu:239-406
+            force.compute(box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
+                          a.virial_per_atom)
+            rec = self.fire_step(box, a)
+            records.append(rec)
+            converged = rec[MIN_CONVERGED] != 0
+            if step == 0 or (step + 1) % base == 0 or converged:
+                lines.append(progress_line(0 if step == 0 else step + 1, rec, self.box_change))
+                if converged:
+                    if self.box_change:
+                        lines.append("  Converged! f_max_atom = %.2e < %.2e AND max_stress = %.2e GPa < %.2e GPa"
+                                     % (rec[MIN_FMAX], self.tol, rec[MIN_STRESS], 1e-4))
+                    break
+        return lines, records
+
+
+def progress_line(step, rec, box_change):
+    """The FIRE progress line (minimizer_fire.cu:132-140, minimizer_fire_box_change.cu:319-327)."""
+    if box_change:
+        return ("    step %d: total_potential = %.10f eV, f_max_atom = %.10f eV/A, pressure = %.6f GPa."
+                % (step, rec[MIN_U], rec[MIN_FMAX], rec[MIN_PRESSURE]))
+    return "    step %d: total_potential = %.10f eV, f_max = %.10f eV/A." % (step, rec[MIN_U], rec[MIN_FMAX])
+
+
 def launch_count():
     return _lib.load().b200md_launch_count()

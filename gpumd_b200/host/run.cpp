@@ -10,13 +10,14 @@
 //   Replicate                                       src/main_gpumd/replicate.cu:20-111
 // Keywords here: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
 // nvt_ber|nvt_nhc|nvt_bdp|nvt_lan|nvt_bao T T tau | npt_ber | heat_lan|heat_nhc|heat_bdp T Tc dT source
-// sink, fix, move, time_step <fs>, run <n>.  The measurement and dump keywords (dump_thermo, dump_xyz,
+// sink, fix, move, time_step <fs>, minimize sd|fire tol steps [box_change [hydrostatic]], run <n>.  The measurement and dump keywords (dump_thermo, dump_xyz,
 // dump_restart, compute, compute_hac, compute_hnemd, compute_shc, compute_dos, compute_sdc,
 // compute_msd) are one Property each in measure.cpp, held by Measure as the reference's Measure holds
 // its properties.  Anything else is an input error (exit 1), as in the reference.
 #include "ensemble.h"
 #include "force.h"
 #include "measure.h"
+#include "minimize.h"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -495,6 +496,8 @@ private:
       if (state_on_gpu_ || has_potential_)
         input_error("replicate must come before 'potential' (run.cu:356-358).");
       replicate(t);
+    } else if (t[0] == "minimize") {
+      minimize(t);
     } else if (t[0] == "run") {
       if (t.size() != 2 || std::atoi(t[1].c_str()) < 0)
         input_error("run should have 1 parameter (the number of steps).");
@@ -506,6 +509,66 @@ private:
     } else {
       input_error("'" + t[0] + "' is not a keyword supported by the b200md backend.");
     }
+  }
+
+  // Minimize::parse_minimize (minimize.cu:32-156), run at parse time with the current `fix` group
+  // (run.cu:359-369); FIRE ignores the group, as the reference
+  void minimize(const std::vector<std::string>& t)
+  {
+    if (!has_potential_)
+      input_error("'potential' must precede 'minimize'.");
+    const int num_param = (int)t.size();
+    int method = 0, steps = 0, box_change = 0, hydrostatic = 0;
+    double tol = 0.0;
+    if (num_param >= 2 && t[1] == "sd") {
+      if (num_param != 4)
+        input_error("minimize sd should have 2 parameters.");
+    } else if (num_param >= 2 && t[1] == "fire") {
+      method = 1;
+      if (!(num_param >= 4 && num_param <= 6))
+        input_error("minimize fire should have 2 to 4 parameters.");
+    } else {
+      input_error("Invalid minimizer.");
+    }
+    if (!valid_real(t[2], &tol))
+      input_error("Force tolerance should be a number.");
+    if (!valid_int(t[3], &steps))
+      input_error("Number of steps should be an integer.");
+    if (steps <= 0)
+      input_error("Number of steps should > 0.");
+    if (num_param >= 5) {
+      if (!valid_int(t[4], &box_change))
+        input_error("Box_change should be an integer.");
+      if (!(box_change == 0 || box_change == 1))
+        input_error("Box_change should be 1 or 0.");
+    }
+    if (num_param >= 6) {
+      if (!valid_int(t[5], &hydrostatic))
+        input_error("Hydrostatic_strain should be an integer.");
+      if (!(hydrostatic == 0 || hydrostatic == 1))
+        input_error("Hydrostatic_strain should be 1 or 0.");
+    }
+    printf("\nStart to do an energy minimization.\n");
+    if (method == 0)
+      printf("    using the steepest descent method.\n");
+    else
+      printf("    using the fast inertial relaxation engine (FIRE) method.\n");
+    if (box_change) {
+      printf("    with variable box.\n");
+      if (hydrostatic)
+        printf("    with hydrostatic pressure.\n");
+    } else {
+      printf("    with fixed box.\n");
+    }
+    printf("    with a force tolerance of %g eV/A.\n", tol);
+    printf("    for maximally %d steps.\n", steps);
+    if (!state_on_gpu_)
+      upload_state();
+    Atom& a = model_.atom;
+    const int* label = (method == 0 && fixed_group_ >= 0) ? model_.group[fixed_method_].label.data() : nullptr;
+    Minimizer_B200 minimizer(method, a.number_of_atoms, steps, tol, box_change, hydrostatic);
+    minimizer.compute(force_, model_.box, a, label, method == 0 ? fixed_group_ : -1);
+    force_.potentials[0]->check();
   }
 
   // Integrate::parse_ensemble, heat branch (integrate.cu:479-493,716-768)

@@ -135,6 +135,14 @@ SIGNATURES = {
     "b200md_nep_set_owned": (C.c_int, [_vp, C.c_int]),
     "b200md_nep_set_accumulate": (C.c_int, [_vp, C.c_int]),
     "b200md_nep_set_active_region": (C.c_int, [_vp, _dp, _dp]),
+    "b200md_minimizer_create": (C.c_int, [C.c_int, C.c_int, C.c_double, C.c_int, C.c_int, C.c_int,
+                                          C.POINTER(_vp)]),
+    "b200md_minimizer_destroy": (None, [_vp]),
+    "b200md_minimizer_velocity": (_vp, [_vp]),
+    "b200md_minimizer_set_record": (C.c_int, [_vp, _dp, _vp]),
+    "b200md_minimizer_sd_begin": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _dp, _vp]),
+    "b200md_minimizer_sd_step": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _dp, _vp]),
+    "b200md_minimizer_fire_step": (C.c_int, [_vp, C.c_int, _dp, _vp, _vp, _vp, _vp, _dp, _vp]),
     "b200md_tc_selftest": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
 }
 

@@ -525,6 +525,78 @@ int b200md_nep_set_accumulate(b200md_nep* p, int accumulate);
  * supercell lie outside the caller's coordinates and need their descriptors. */
 int b200md_nep_set_active_region(b200md_nep* p, const double lo[3], const double hi[3]);
 
+/* ------------------------------------------------------------------------------------------
+ * Energy minimization.  Replaces Minimize::parse_minimize's minimizers (src/minimize/minimize.cu:32-156):
+ *   b200md_minimizer_create     <- Minimizer_SD / Minimizer_FIRE / Minimizer_FIRE_Box_Change constructors
+ *                                  (minimizer.cuh:27-50, minimizer_fire.cuh:24-45,
+ *                                  minimizer_fire_box_change.cuh:24-53).  method 0 sd, 1 fire; box_change
+ *                                  and hydrostatic (0 / 1) for fire only.  The handle owns the FIRE velocity
+ *                                  (zero at creation), the control record and the reduction scratch; nothing
+ *                                  is allocated after creation.
+ *   b200md_minimizer_sd_begin   <- the start of Minimizer_SD::compute (minimizer_sd.cu:77-118): call after the
+ *                                  first force evaluation of (d_position, d_force, d_potential).  Reduces f_max
+ *                                  and sum U, then writes the trial positions x + F step / f_max to
+ *                                  d_position_trial (the atoms of label fixed_group keep x; fixed_group -1 and
+ *                                  d_group_label NULL: none).  The caller evaluates the force at the trial
+ *                                  positions into d_force_trial / d_potential_trial (the reference's _temp
+ *                                  vectors, minimizer.cuh:38-40; caller-owned, 3n / 3n / n doubles).
+ *   b200md_minimizer_sd_step    <- the rest of one SD iteration (minimizer_sd.cu:122-137): sum U_trial; uphill
+ *                                  (U_trial > U) -> step *= 0.2, else the trial x, F, U are copied over the
+ *                                  caller's on the device and step *= 1.2; then f_max and sum U of the new
+ *                                  state and the next trial positions.
+ *   b200md_minimizer_fire_step  <- one iteration of Minimizer_FIRE::compute (minimizer_fire.cu:108-180) or
+ *                                  Minimizer_FIRE_Box_Change::compute (minimizer_fire_box_change.cu:239-406),
+ *                                  after the caller's force evaluation: f_max, sum U, P = v.F, |F|, |v| (and the
+ *                                  virial box force) in one reduction, the FIRE control step on the device, and
+ *                                  one update pass over the atoms (nothing moves once converged).  Box change:
+ *                                  h[9] (HOST) is updated in place to h + dEps h, as b200md_berendsen_pressure
+ *                                  does, and L = cbrt(volume) is taken from h at the first call.
+ * Each call writes the handle's record (B200MD_MIN_RECORD doubles) to `record` (host, may be NULL for the SD
+ * calls): the only device-to-host copy of an iteration, which synchronises the stream.
+ *   b200md_minimizer_velocity    the FIRE velocity, device double[3n] (SoA)
+ *   b200md_minimizer_set_record  test hook: overwrite the record (the control state dt, alpha, N_neg, step,
+ *                                v_box and, when > 0, L)
+ * ------------------------------------------------------------------------------------------ */
+#define B200MD_MIN_FMAX 0      /* sqrt(max F_i^2) over the atom force components of the current state */
+#define B200MD_MIN_U 1         /* sum U of the current state (eV) */
+#define B200MD_MIN_CONVERGED 2 /* 1: f_max < tol (box change: and the stress below 1e-4 GPa) */
+#define B200MD_MIN_DT 3        /* FIRE time step (natural units) after the control step */
+#define B200MD_MIN_ALPHA 4
+#define B200MD_MIN_NNEG 5      /* FIRE's count of P > 0 iterations since the last uphill one */
+#define B200MD_MIN_P 6         /* v.F before the control step (box change: over the 3N + 9 entries) */
+#define B200MD_MIN_FMOD 7      /* |F| (generalized for box change) */
+#define B200MD_MIN_VMOD 8      /* |v| after the possible zeroing, before the kick */
+#define B200MD_MIN_UPHILL 9    /* FIRE: P <= 0 branch taken; SD: the trial was rejected */
+#define B200MD_MIN_PRESSURE 10 /* box change: trace of the stress / 3 (GPa) */
+#define B200MD_MIN_STRESS 11   /* box change: max |stress component| (hydrostatic: |pressure|), GPa */
+#define B200MD_MIN_STEP 12     /* SD position step (starts at 0.1) */
+#define B200MD_MIN_UTRIAL 13   /* SD: sum U at the trial positions */
+#define B200MD_MIN_USMALLER 14 /* SD: the lower of sum U and sum U_trial of the last decision */
+#define B200MD_MIN_SCALE 15    /* FIRE: alpha |v| / |F|; SD: step / f_max */
+#define B200MD_MIN_LSCALE 16   /* box change: L = cbrt(V0) */
+#define B200MD_MIN_DEPS 17     /* box change: dEps[9] = v_box dt / L, row-major */
+#define B200MD_MIN_VBOX 26     /* box change: v_box[9] */
+#define B200MD_MIN_FBOX 35     /* box change: the box force[9] = virial / L (hydrostatic: trace / 3) */
+#define B200MD_MIN_RECORD 44
+typedef struct b200md_minimizer b200md_minimizer;
+int b200md_minimizer_create(
+  int method, int n, double force_tolerance, int number_of_steps, int box_change, int hydrostatic,
+  b200md_minimizer** out);
+void b200md_minimizer_destroy(b200md_minimizer* p);
+double* b200md_minimizer_velocity(b200md_minimizer* p);
+int b200md_minimizer_set_record(b200md_minimizer* p, const double* record, void* stream);
+int b200md_minimizer_sd_begin(
+  b200md_minimizer* p, int n, double* d_position, double* d_force, double* d_potential,
+  double* d_position_trial, const double* d_force_trial, const double* d_potential_trial,
+  const int* d_group_label, int fixed_group, double* record, void* stream);
+int b200md_minimizer_sd_step(
+  b200md_minimizer* p, int n, double* d_position, double* d_force, double* d_potential,
+  double* d_position_trial, const double* d_force_trial, const double* d_potential_trial,
+  const int* d_group_label, int fixed_group, double* record, void* stream);
+int b200md_minimizer_fire_step(
+  b200md_minimizer* p, int n, double h[9], double* d_position, const double* d_force,
+  const double* d_potential, const double* d_virial, double* record, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Tensor-core self-test (no reference counterpart): one CTA computes D[128 x N] = A[128 x K] .
  * B[N x K]^T on the tensor cores (one warpgroup, wgmma.mma_async tf32, 3xTF32 split, FP32

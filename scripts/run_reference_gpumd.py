@@ -50,6 +50,51 @@ CORR_GRAPHENE_RUNS = {
 CORR_SI_RUN = "time_step 2\nensemble nve\ncompute_sdc 2 100\ncompute_msd 2 100 save_every 300\nrun 400\n"
 
 
+# energy minimization: `minimize ...` followed by the single-point tail; tests/test_gpu_minimize.py runs the
+# same inputs through the b200md driver.  case: (structure, symbols (None: the NEP file's order), potential
+# file, lines before `minimize` and the `minimize` line, head before `potential`, model.xyz to copy)
+MIN_TAIL = "velocity 1\nensemble nve\ntime_step 0\ndump_xyz 1 dump.xyz precision double force\nrun 1\n"
+
+
+def _min_si(group=False):
+    from gpumd_b200.structures import diamond
+    s = diamond(4, a=5.431, rattle=0.05, seed=31)  # 512 atoms
+    if group:  # group 0: every fourth atom
+        s["group"] = (np.arange(s["type"].shape[0]) % 4 != 0).astype(np.int32)
+    return s
+
+
+def _min_pbte():
+    s = rocksalt_pbte(4, rattle=0.03, seed=32)  # 512 atoms, strained by -2 %
+    return dict(s, h=s["h"] * 0.98, pos=s["pos"] * 0.98)
+
+
+MIN_CASES = {
+    "min_si_sd": (_min_si, ["Si"], "tersoff_Si_1989.txt", "minimize sd 1.0e-4 1000\n", "", None),
+    "min_si_sd_fix": (lambda: _min_si(True), ["Si"], "tersoff_Si_1989.txt", "fix 0\nminimize sd 1.0e-4 1000\n",
+                      "", None),
+    "min_si_fire": (_min_si, ["Si"], "tersoff_Si_1989.txt", "minimize fire 1.0e-4 1000\n", "", None),
+    "min_si_fire_fix": (lambda: _min_si(True), ["Si"], "tersoff_Si_1989.txt",
+                        "fix 0\nminimize fire 1.0e-4 1000\n", "", None),
+    # 50 iterations: further on this rattled, compressed cell rearranges into a much denser structure (about
+    # 0.8 eV/atom lower after 1000 iterations, in the reference too), where FP32 rounding decides the path
+    "min_pbte_fire_box": (_min_pbte, None, "nep_PbTe.txt", "minimize fire 1.0e-4 50 1\n", "", None),
+    "min_pbte_fire_box_hydro": (_min_pbte, None, "nep_PbTe.txt", "minimize fire 1.0e-4 50 1 1\n", "", None),
+    "min_lj_fire": (lambda: fcc(6, 5.26, rattle=0.1, seed=33), ["Ar"], "lj_Ar_10A.txt",
+                    "minimize fire 1.0e-4 1000\n", "", None),
+    "min_eam_sd": (lambda: fcc(7, 3.615, rattle=0.05, seed=34, symbols=("Cu",)), ["Cu"], "eam_Cu_Zhou_2004.txt",
+                   "minimize sd 1.0e-4 1000\n", "", None),
+    # the reference's tests/gpumd/silicon_dispersion recipe (its two-atom cell, replicated 6 x 6 x 6)
+    "min_si_dispersion": (None, ["Si"], "tersoff_Si_1989.txt", "minimize sd 1.0e-6 10000\n", "replicate 6 6 6\n",
+                          GOLDEN / "silicon_dispersion_model.xyz"),
+}
+
+
+def min_progress(stdout):
+    """The minimizer's progress lines of a gpumd / b200md stdout."""
+    return [ln for ln in stdout.splitlines() if ln.startswith(("    step ", "    Position step", "  Converged!"))]
+
+
 def write_model(path, s, symbols, vel=None):
     write_xyz(path, s, symbols, vel)
 
@@ -57,10 +102,10 @@ def write_model(path, s, symbols, vel=None):
 ONLY = None  # --only REGEX: run just the matching cases
 
 
-def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1, model_file=None):
+def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1, model_file=None, head=""):
     """gpus > 1: that many visible devices -> the reference takes its NEP_MULTIGPU path
     (src/force/force.cu:139-160); skipped when the box has fewer.  model_file: copy this model.xyz
-    instead of writing one from s."""
+    instead of writing one from s.  head: keywords before the `potential` line (replicate)."""
     if ONLY and not re.search(ONLY, name):
         return None, None
     import os
@@ -83,7 +128,7 @@ def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1,
         write_model(d / "model.xyz", s, symbols, vel)
     else:
         shutil.copyfile(model_file, d / "model.xyz")
-    (d / "run.in").write_text("potential potential.txt\n" + run_in)
+    (d / "run.in").write_text(head + "potential potential.txt\n" + run_in)
     t0 = time.time()
     r = subprocess.run([str(BIN)], cwd=d, capture_output=True, text=True, timeout=timeout, env=env)
     wall = time.time() - t0
@@ -107,6 +152,16 @@ def collect_single_point(d, s, symbols):
     (d / "dump.xyz").unlink()
 
 
+def collect_minimize(d, name):
+    """-> refgpu_out/refgpu_<name>_progress.txt (the progress lines) and refgpu_<name>_dump.xyz.gz"""
+    if d is None:
+        return
+    import gzip
+    text = (d / "stdout.txt").read_text()
+    (OUT / f"refgpu_{name}_progress.txt").write_text("\n".join(min_progress(text)) + "\n")
+    (OUT / f"refgpu_{name}_dump.xyz.gz").write_bytes(gzip.compress((d / "dump.xyz").read_bytes(), mtime=0))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--skip-speed", action="store_true")
@@ -119,6 +174,13 @@ def main():
     OUT.mkdir(parents=True, exist_ok=True)
     infos = []
     sp = "velocity 1\nensemble nve\ntime_step 0\ndump_xyz 1 dump.xyz precision double force\nrun 1\n"
+
+    # ---- (0) energy minimization ----
+    for name, (make, symbols, pot, lines, head, model_file) in MIN_CASES.items():
+        sym = symbols or nep_type_order(GOLDEN / pot)
+        s = make() if make else None
+        d, i = run_case(name, s, sym, GOLDEN / pot, lines + MIN_TAIL, model_file=model_file, head=head)
+        collect_minimize(d, name); infos.append(i)
 
     # ---- (1) single points on the large-box path ----
     pbte_sym = nep_type_order(GOLDEN / "nep_PbTe.txt")
