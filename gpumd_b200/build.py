@@ -19,7 +19,7 @@ OBJ = PKG / "build"
 
 CU_SOURCES = ["b2_host.cu", "b2_neighbor.cu", "b2_nep.cu", "b2_md.cu", "b2_tersoff.cu", "b2_eam.cu",
               "b2_tc_test.cu", "b2_stochastic.cu", "b2_measure.cu", "b2_nemd.cu", "b2_correlate.cu",
-              "b2_minimize.cu"]
+              "b2_minimize.cu", "b2_phonon.cu"]
 CPP_SOURCES = ["b2_nep_model.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -104,7 +104,7 @@ def build_host(force=False):
     """The C++ host layer (adapter classes + standalone driver) -> gpumd_b200/b200md."""
     nvcc = _nvcc()
     srcs = [HOST / f for f in ("potential.cpp", "force.cpp", "ensemble.cpp", "measure.cpp", "minimize.cpp",
-                                       "run.cpp")]
+                                       "phonon.cpp", "run.cpp")]
     deps = srcs + list(HOST.glob("*.h")) + [PKG.parent / "include" / "b200md.h", LIB]
     if force or _stale(EXE, deps):
         cmd = [nvcc, "-O2", "-std=c++17", "-x", "cu", "-gencode", "arch=compute_90a,code=sm_90a"] + \

@@ -1140,3 +1140,145 @@ def progress_line(step, rec, box_change):
 
 def launch_count():
     return _lib.load().b200md_launch_count()
+
+
+PI = 3.14159265358979  # src/utilities/common.cuh:20
+NATURAL_TO_THZ2 = 1.0e6 / (TIME_UNIT_CONVERSION * TIME_UNIT_CONVERSION)  # hessian.cu:352, omega^2 in THz^2
+
+
+def box_inverse(h):
+    """cpu_h[9..17] of Box::get_inverse (src/model/box.cu:60-78): adjugate over determinant, in its order."""
+    h = [float(x) for x in np.asarray(h, dtype=np.float64).reshape(9)]
+    a = [h[4] * h[8] - h[5] * h[7], h[2] * h[7] - h[1] * h[8], h[1] * h[5] - h[2] * h[4],
+         h[5] * h[6] - h[3] * h[8], h[0] * h[8] - h[2] * h[6], h[2] * h[3] - h[0] * h[5],
+         h[3] * h[7] - h[4] * h[6], h[1] * h[6] - h[0] * h[7], h[0] * h[4] - h[1] * h[3]]
+    det = h[0] * a[0] + h[1] * a[3] + h[2] * a[6]
+    return np.array([x / det for x in a])
+
+
+def kpoint_path(segments, box, cxyz):
+    """Hessian::create_kpoints (src/phonon/hessian.cu:110-198) after parsing: segments is a list of lists of
+    fractional k-points of the primitive cell.  Returns (kpoints [nk, 3] Cartesian, kpath [nk], kpath at
+    each high-symmetry point).  Every leg is split into 100 points; the jump between segments is not
+    counted."""
+    inv = box_inverse(box.cpu_h).reshape(3, 3)
+    rec = np.empty((3, 3))
+    for i in range(3):
+        for j in range(3):
+            rec[j][i] = 2.0 * PI * cxyz[i] * inv[i][j]
+
+    def mv(k):
+        return [rec[r][0] * k[0] + rec[r][1] * k[1] + rec[r][2] * k[2] for r in range(3)]
+
+    nk = (1 - len(segments) + sum(len(s) for s in segments) - 1) * 100 + 1
+    kpts, kpath, ksym = [mv(segments[0][0])], [0.0], [0.0]
+    length = 0.0
+    for seg in segments:
+        for i in range(1, len(seg)):
+            start, end = mv(seg[i - 1]), mv(seg[i])
+            last = start
+            for j in range(1, 101):
+                t = j * 0.01
+                k = [start[c] + t * (end[c] - start[c]) for c in range(3)]
+                d = [k[c] - last[c] for c in range(3)]
+                length += float(np.sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]))
+                kpts.append(k)
+                kpath.append(length)
+                last = k
+                if j == 100:
+                    ksym.append(length)
+    assert len(kpts) == nk
+    return np.array(kpts, dtype=np.float64).reshape(nk, 3), np.array(kpath), np.array(ksym)
+
+
+class Phonon:
+    """`compute_phonon displacement`, Hessian::compute (src/phonon/hessian.cu:65-81), with the force constants
+    from 6 * num_basis force calls (each basis atom displaced by -d and +d along x, y, z; the forces on every
+    atom give its row of H) and D(k), the eigenvalues and, at a single k-point, the eigenvectors on the device.
+
+    compute(force, box, atom, cxyz, segments) uses the current positions and box; num_basis =
+    N / (cx cy cz), atom n has the label n % num_basis.  Returns a dict: H [num_basis, N, 9], D [nk, dim, dim]
+    complex (D[k, row, col]), kpoints, kpath, kpath_sym, omega2 [nk, dim] in THz^2 (ascending), cutoff, and
+    with one k-point eigenvectors [dim, dim] (columns).  The positions are left bit for bit as they were."""
+
+    def __init__(self, displacement):
+        _require_cuda()
+        self._L = _lib.load()
+        self.displacement = float(displacement)
+
+    def compute(self, force, box, atom, cxyz, segments, sweep_hook=None):
+        n = atom.number_of_atoms
+        cutoff = 2.0 * max(p.rc for p in force.potentials)
+        num_basis = n // (int(cxyz[0]) * int(cxyz[1]) * int(cxyz[2]))
+        kpts, kpath, ksym = kpoint_path(segments, box, cxyz)
+        nk = kpts.shape[0]
+        kp = np.ascontiguousarray(kpts.reshape(-1))
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_phonon_create(n, num_basis, nk, kp.ctypes.data_as(C.POINTER(C.c_double)),
+                                                self.displacement, C.byref(h)))
+        try:
+            st = _stream()
+            a = atom
+            _lib.check(self._L.b200md_phonon_begin(h, n, box._h, box._p, cutoff, _ptr(a.position_per_atom),
+                                                   _ptr(a.mass), st))
+            for call in range(6 * num_basis):
+                force.compute(box, a.position_per_atom, a.type, a.potential_per_atom, a.force_per_atom,
+                              a.virial_per_atom)
+                if sweep_hook is not None:
+                    sweep_hook(call)
+                _lib.check(self._L.b200md_phonon_step(h, call, _ptr(a.position_per_atom), _ptr(a.force_per_atom),
+                                                      st))
+            _lib.check(self._L.b200md_phonon_dynamical(h, st))
+            _lib.check(self._L.b200md_phonon_eig(h, st))
+            dim = 3 * num_basis
+            out = dict(cutoff=cutoff, num_basis=num_basis, kpoints=kpts, kpath=kpath, kpath_sym=ksym)
+            out["H"] = phonon_read(h, PHONON_H, num_basis * n * 9).reshape(num_basis, n, 9)
+            # column-major per k-point: [k, col, row] -> D[k, row, col]
+            D = phonon_read(h, PHONON_D_REAL, nk * dim * dim).reshape(nk, dim, dim)
+            if nk > 1:
+                D = D + 1j * phonon_read(h, PHONON_D_IMAG, nk * dim * dim).reshape(nk, dim, dim)
+            out["D"] = np.ascontiguousarray(D.transpose(0, 2, 1))
+            out["omega2"] = phonon_read(h, PHONON_W, nk * dim).reshape(nk, dim) * NATURAL_TO_THZ2
+            if nk == 1:
+                out["eigenvectors"] = phonon_read(h, PHONON_V, dim * dim).reshape(dim, dim).T
+            return out
+        finally:
+            self._L.b200md_phonon_destroy(h)
+
+
+PHONON_H, PHONON_D_REAL, PHONON_D_IMAG, PHONON_W, PHONON_V = range(5)  # b200md_phonon_read (include/b200md.h)
+
+
+def phonon_read(handle, what, count):
+    """One array of a b200md_phonon handle -> numpy (b200md_phonon_read copies it and synchronises)."""
+    out = np.empty(count, dtype=np.float64)
+    _lib.check(_lib.load().b200md_phonon_read(handle, what, out.ctypes.data_as(C.POINTER(C.c_double)), _stream()))
+    return out
+
+
+def jacobi_eig(re, im=None, vectors=False):
+    """b200md_jacobi_eig on a batch of dim x dim matrices (numpy [batch, dim, dim], row index first); the lower
+    triangle is read.  Hermitian when im is given (eigenvalues only), else real symmetric, with eigenvectors
+    (columns) when vectors.  Returns w [batch, dim] ascending (and v [batch, dim, dim]); raises when a matrix is
+    not diagonal after the solver's sweep cap."""
+    _require_cuda()
+    L = _lib.load()
+    re = np.asarray(re, dtype=np.float64)
+    b, dim = re.shape[0], re.shape[1]
+    z = dict(dtype=torch.float64, device="cuda")
+    # column-major per matrix: [batch, col, row]
+    dre = torch.as_tensor(np.ascontiguousarray(re.transpose(0, 2, 1)), **z)
+    dim_t = None if im is None else torch.as_tensor(
+        np.ascontiguousarray(np.asarray(im, dtype=np.float64).transpose(0, 2, 1)), **z)
+    w = torch.empty(b * dim, **z)
+    v = torch.empty(b * dim * dim, **z) if vectors else None
+    info = torch.empty(b, dtype=torch.int32, device="cuda")
+    _lib.check(L.b200md_jacobi_eig(dim, b, 0 if im is None else 1, _ptr(dre),
+                                   None if dim_t is None else _ptr(dim_t), _ptr(w), None if v is None else _ptr(v),
+                                   _ptr(info), _stream()))
+    if (info < 0).any():
+        raise _lib.B200mdError(f"b200md_jacobi_eig did not converge for matrices {torch.nonzero(info < 0).tolist()}")
+    wn = w.cpu().numpy().reshape(b, dim)
+    if not vectors:
+        return wn
+    return wn, v.cpu().numpy().reshape(b, dim, dim).transpose(0, 2, 1)

@@ -10,7 +10,8 @@
 //   Replicate                                       src/main_gpumd/replicate.cu:20-111
 // Keywords here: replicate <na nb nc>, potential, velocity <T> [seed <s>], ensemble nve |
 // nvt_ber|nvt_nhc|nvt_bdp|nvt_lan|nvt_bao T T tau | npt_ber | heat_lan|heat_nhc|heat_bdp T Tc dT source
-// sink, fix, move, time_step <fs>, minimize sd|fire tol steps [box_change [hydrostatic]], run <n>.  The measurement and dump keywords (dump_thermo, dump_xyz,
+// sink, fix, move, time_step <fs>, minimize sd|fire tol steps [box_change [hydrostatic]],
+// compute_phonon <displacement>, run <n>.  The measurement and dump keywords (dump_thermo, dump_xyz,
 // dump_restart, compute, compute_hac, compute_hnemd, compute_shc, compute_dos, compute_sdc,
 // compute_msd) are one Property each in measure.cpp, held by Measure as the reference's Measure holds
 // its properties.  Anything else is an input error (exit 1), as in the reference.
@@ -18,6 +19,7 @@
 #include "force.h"
 #include "measure.h"
 #include "minimize.h"
+#include "phonon.h"
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -319,6 +321,9 @@ private:
   double global_time_ = 0.0; // natural units, as Run::global_time (run.cu:316)
   bool state_on_gpu_ = false;
   bool has_potential_ = false;
+  // the product of the factors of every `replicate` line, wherever it stands (compute_phonon's cell)
+  int replicate_[3] = {1, 1, 1};
+  bool has_replicate_ = false;
   Measure measure_;
   const MeasureContext ctx_{model_,       force_,   ensemble_,    time_step_,    global_time_,
                             temperature_, thermo_,  fixed_group_, fixed_method_, unwrapped_};
@@ -498,6 +503,8 @@ private:
       replicate(t);
     } else if (t[0] == "minimize") {
       minimize(t);
+    } else if (t[0] == "compute_phonon") {
+      compute_phonon(t);
     } else if (t[0] == "run") {
       if (t.size() != 2 || std::atoi(t[1].c_str()) < 0)
         input_error("run should have 1 parameter (the number of steps).");
@@ -569,6 +576,20 @@ private:
     Minimizer_B200 minimizer(method, a.number_of_atoms, steps, tol, box_change, hydrostatic);
     minimizer.compute(force_, model_.box, a, label, method == 0 ? fixed_group_ : -1);
     force_.potentials[0]->check();
+  }
+
+  // run.cu:370-373: Hessian::parse + Hessian::compute at parse time, on the current positions and box
+  void compute_phonon(const std::vector<std::string>& t)
+  {
+    Hessian_B200 hessian;
+    hessian.parse(t);
+    if (!has_potential_)
+      input_error("'potential' must precede 'compute_phonon'.");
+    if (!has_replicate_)
+      input_error("replicate keyword not found in run.in file.");
+    if (!state_on_gpu_)
+      upload_state();
+    hessian.compute(force_, model_.box, model_.atom, replicate_);
   }
 
   // Integrate::parse_ensemble, heat branch (integrate.cu:479-493,716-768)
@@ -647,6 +668,9 @@ private:
     a.cpu_position_per_atom.swap(pos);
     a.cpu_velocity_per_atom.swap(vel);
     printf("Replicate cell by %d * %d * %d.\nNumber of atoms is %d.\n", r[0], r[1], r[2], N);
+    for (int d = 0; d < 3; ++d)
+      replicate_[d] *= r[d];
+    has_replicate_ = true;
   }
 
   // Integrate::initialize: a fresh ensemble object per run, from the CURRENT time step

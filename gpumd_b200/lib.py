@@ -143,6 +143,14 @@ SIGNATURES = {
     "b200md_minimizer_sd_begin": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _dp, _vp]),
     "b200md_minimizer_sd_step": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int, _dp, _vp]),
     "b200md_minimizer_fire_step": (C.c_int, [_vp, C.c_int, _dp, _vp, _vp, _vp, _vp, _dp, _vp]),
+    "b200md_phonon_create": (C.c_int, [C.c_int, C.c_int, C.c_int, _dp, C.c_double, C.POINTER(_vp)]),
+    "b200md_phonon_destroy": (None, [_vp]),
+    "b200md_phonon_begin": (C.c_int, [_vp, C.c_int, _dp, _ip, C.c_double, _vp, _vp, _vp]),
+    "b200md_phonon_step": (C.c_int, [_vp, C.c_int, _vp, _vp, _vp]),
+    "b200md_phonon_dynamical": (C.c_int, [_vp, _vp]),
+    "b200md_phonon_eig": (C.c_int, [_vp, _vp]),
+    "b200md_phonon_read": (C.c_int, [_vp, C.c_int, _dp, _vp]),
+    "b200md_jacobi_eig": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200md_tc_selftest": (C.c_int, [C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp]),
 }
 

@@ -31,6 +31,7 @@ extern "C" {
 #define B200MD_ERR_CUDA 3      /* CUDA runtime error */
 #define B200MD_ERR_SMALL_BOX 4 /* periodic thickness <= 2.5*(rc+1): reference's small-box path */
 #define B200MD_ERR_OVERFLOW 5  /* neighbour / cell capacity exceeded on the device */
+#define B200MD_ERR_NOT_CONVERGED 6 /* an iterative solver reached its iteration cap */
 
 const char* b200md_last_error(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
@@ -596,6 +597,68 @@ int b200md_minimizer_sd_step(
 int b200md_minimizer_fire_step(
   b200md_minimizer* p, int n, double h[9], double* d_position, const double* d_force,
   const double* d_potential, const double* d_virial, double* record, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Harmonic phonons.  Replaces Hessian::compute (src/phonon/hessian.cu:65-81):
+ *   b200md_phonon_create     <- Hessian::initialize's allocations (hessian.cu:200-253): n atoms, num_basis
+ *                               basis atoms (atoms 0 .. num_basis-1; atom n has the label n % num_basis),
+ *                               num_kpoints Cartesian k-points kpoints[3 * num_kpoints] (1 / A), the
+ *                               displacement d (A).  1 <= num_basis <= B200MD_PHONON_MAX_BASIS.
+ *   b200md_phonon_begin      <- the start of Hessian::find_H (hessian.cu:272-302): saves the positions and the
+ *                               num_basis masses, computes r12 = x[n2] - x[n1] under the minimum image of
+ *                               box (h, pbc) for every basis atom n1 and atom n2 and the mask r12^2 <= cutoff^2
+ *                               (Hessian::is_too_far, hessian.cu:255-270), then displaces the position for the
+ *                               first force call.
+ *   b200md_phonon_step       <- find_H12 (src/force/force_constant.cu:80-133), one step per force call
+ *                               call = 0 .. 6 num_basis - 1, made with the positions the previous step left.
+ *                               Call j displaces basis atom j / 6 along a = (j % 6) / 2 by -d (j even) or +d
+ *                               (j odd); one kernel keeps F(-) or writes H[n1][n2][a*3+b] =
+ *                               (F_n2^b(-) - F_n2^b(+)) / 2d (0 beyond the cutoff), then sets the position for
+ *                               the next call from the saved copy.  After the last call the positions are the
+ *                               saved ones, bit for bit.  No host synchronisation.
+ *   b200md_phonon_dynamical  <- the D(k) sums of find_dispersion (hessian.cu:391-419); with one k-point those
+ *                               of find_D (hessian.cu:431-458): real, no phase.  D is column-major per k-point
+ *                               (entry (row, col) at k * dim^2 + col * dim + row, dim = 3 num_basis).
+ *   b200md_phonon_eig        <- eig_hermitian_Jacobi_batch / eig_hermitian_QR (hessian.cu:347-374): the
+ *                               eigenvalues of every D(k) from its lower triangle, ascending; with one k-point
+ *                               eigenvectors_symmetric_Jacobi (hessian.cu:460-492): eigenvalues and
+ *                               eigenvectors of the real D.  Natural units (eV / A^2 / amu).  Synchronises the
+ *                               stream and returns B200MD_ERR_NOT_CONVERGED when a matrix is not diagonal after
+ *                               the solver's sweep cap.
+ *   b200md_phonon_read       copies one array to host memory and synchronises the stream.  what:
+ *                               B200MD_PHONON_H  H [num_basis][n][9];
+ *                               B200MD_PHONON_D_REAL, _D_IMAG  D [num_kpoints][dim][dim], column-major per k-point
+ *                                 (the imaginary part for num_kpoints > 1 only);
+ *                               B200MD_PHONON_W  eigenvalues [num_kpoints][dim];
+ *                               B200MD_PHONON_V  eigenvectors [dim][dim], column-major, as columns
+ *                                 (num_kpoints == 1 only).
+ *   b200md_jacobi_eig        the eigensolver on `batch` column-major dim x dim matrices (lower triangle
+ *                            read): hermitian 1 -> eigenvalues d_w[batch][dim] of re + i im; hermitian 0 ->
+ *                            eigenvalues of re and, when d_v is given, eigenvectors d_v[batch][dim][dim].
+ *                            d_info[batch] (device) gets the sweeps each matrix took, or -1 when it was not
+ *                            diagonal after the sweep cap.  One CTA per matrix, cyclic Jacobi in shared memory;
+ *                            1 <= dim <= 96.  Asynchronous.
+ * ------------------------------------------------------------------------------------------- */
+#define B200MD_PHONON_MAX_BASIS 32
+typedef struct b200md_phonon b200md_phonon;
+int b200md_phonon_create(
+  int n, int num_basis, int num_kpoints, const double* kpoints, double displacement, b200md_phonon** out);
+void b200md_phonon_destroy(b200md_phonon* p);
+int b200md_phonon_begin(
+  b200md_phonon* p, int n, const double h[9], const int pbc[3], double cutoff, double* d_position,
+  const double* d_mass, void* stream);
+int b200md_phonon_step(b200md_phonon* p, int call, double* d_position, const double* d_force, void* stream);
+int b200md_phonon_dynamical(b200md_phonon* p, void* stream);
+int b200md_phonon_eig(b200md_phonon* p, void* stream);
+#define B200MD_PHONON_H 0
+#define B200MD_PHONON_D_REAL 1
+#define B200MD_PHONON_D_IMAG 2
+#define B200MD_PHONON_W 3
+#define B200MD_PHONON_V 4
+int b200md_phonon_read(b200md_phonon* p, int what, double* host, void* stream);
+int b200md_jacobi_eig(
+  int dim, int batch, int hermitian, const double* d_re, const double* d_im, double* d_w, double* d_v,
+  int* d_info, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Tensor-core self-test (no reference counterpart): one CTA computes D[128 x N] = A[128 x K] .

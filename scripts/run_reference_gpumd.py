@@ -90,6 +90,82 @@ MIN_CASES = {
 }
 
 
+# phonons: `compute_phonon` at parse time (after `minimize` for silicon_dispersion); tests/test_gpu_phonon.py runs
+# the same inputs through the b200md driver.  case: (structure of the replicated cell, or None with model_file;
+# symbols (None: the NEP file's order); potential file; `replicate` line; lines after `potential`; model.xyz to
+# copy; kpoints.in; whether D.out is kept (the cells of at most two atoms: larger ones exceed 1 MB))
+FCC_PATH = "0 0 0 G\n0.5 0 0.5 X\n0.375 0.375 0.75 K\n0 0 0 G\n0.5 0.5 0.5 L\n"
+
+
+def fcc_primitive(a, symbols, basis=((0.0, 0.0, 0.0),)):
+    """The primitive fcc cell (lattice vectors a/2 (0,1,1), (1,0,1), (1,1,0)) with atoms at the given
+    fractions of the cubic edge a."""
+    h = 0.5 * a * np.array([[0, 1, 1], [1, 0, 1], [1, 1, 0]], dtype=float)  # columns
+    pos = a * np.array(basis, dtype=float).T
+    from gpumd_b200.structures import MASS
+    return dict(h=h.reshape(9), pbc=np.array([1, 1, 1]), pos=pos, type=np.arange(len(basis), dtype=np.int32),
+                mass=np.array([MASS[symbols[t]] for t in range(len(basis))]))
+
+
+def fcc_two_atom(a, symbol):
+    """fcc in its two-atom tetragonal cell: lattice vectors (a/2)(1,1,0), (a/2)(-1,1,0), (0,0,a), atoms at 0 and
+    (a/2)(1,0,1) (the reference reads no model of fewer than two atoms)."""
+    from gpumd_b200.structures import MASS
+    h = np.array([[0.5 * a, -0.5 * a, 0.0], [0.5 * a, 0.5 * a, 0.0], [0.0, 0.0, a]])  # columns
+    pos = np.array([[0.0, 0.5 * a], [0.0, 0.0], [0.0, 0.5 * a]])
+    return dict(h=h.reshape(9), pbc=np.array([1, 1, 1]), pos=pos, type=np.zeros(2, np.int32),
+                mass=np.full(2, MASS[symbol]))
+
+
+def _zincblende_sic():
+    from gpumd_b200.structures import diamond
+    s = diamond(1, a=4.36)
+    s["type"] = np.array([0, 0, 0, 0, 1, 1, 1, 1], np.int32)
+    return s
+
+
+def _diamond(reps):
+    from gpumd_b200.structures import diamond
+    return lambda: diamond(reps)
+
+
+PHONON_CASES = {
+    # the reference's tests/gpumd/silicon_dispersion input, exactly
+    "phonon_si_dispersion": (None, ["Si"], "tersoff_Si_1989.txt", "replicate 6 6 6\n",
+                             "minimize sd 1.0e-6 10000\ncompute_phonon 0.005\n", GOLDEN / "silicon_dispersion_model.xyz",
+                             (GOLDEN / "ref_silicon_dispersion_kpoints.in").read_text(), True),
+    # two masses, two k-path segments (the '|' header)
+    "phonon_sic": (_zincblende_sic, ["Si", "C"], "tersoff_SiC_1989.txt", "replicate 3 3 3\n", "compute_phonon 0.005\n",
+                   None, "0 0 0 G\n0.5 0 0.5 X\n\n0.5 0.5 0.5 L\n0 0 0 G\n", False),
+    "phonon_pbte": (lambda: fcc_primitive(6.57, ["Te", "Pb"], ((0, 0, 0), (0.5, 0.5, 0.5))), None, "nep_PbTe.txt",
+                    "replicate 6 6 6\n", "compute_phonon 0.005\n", None, FCC_PATH, True),
+    "phonon_lj": (lambda: fcc_two_atom(5.26, "Ar"), ["Ar"], "lj_Ar_10A.txt", "replicate 8 8 6\n",
+                  "compute_phonon 0.005\n", None, "0 0 0 G\n0.5 0 0 X\n0.5 0.5 0.5 R\n", True),
+    "phonon_eam": (lambda: fcc_two_atom(3.615, "Cu"), ["Cu"], "eam_Cu_Zhou_2004.txt", "replicate 8 8 6\n",
+                   "compute_phonon 0.005\n", None, "0 0 0 G\n0.5 0 0 X\n0.5 0.5 0.5 R\n", True),
+    # 16 basis atoms: the reference's per-k-point zheevd branch (more than 10)
+    "phonon_si16": (_diamond((2, 1, 1)), ["Si"], "tersoff_Si_1989.txt", "replicate 2 3 3\n", "compute_phonon 0.005\n",
+                    None, "0 0 0 G\n0.5 0 0 X\n", False),
+    # one k-point: eigenvector.out
+    "phonon_gamma": (_diamond(1), ["Si"], "tersoff_Si_1989.txt", "replicate 2 2 2\n", "compute_phonon 0.005\n",
+                     None, "0 0 0 G\n", False),
+}
+
+
+def collect_phonon(d, name, keep_d):
+    """-> refgpu_out/refgpu_<name>_omega2.out, _D.out.gz, _eigenvector.out (those the run wrote)"""
+    if d is None:
+        return
+    import gzip
+    if (d / "omega2.out").exists():
+        shutil.copyfile(d / "omega2.out", OUT / f"refgpu_{name}_omega2.out")
+    if keep_d and (d / "D.out").exists():
+        (OUT / f"refgpu_{name}_D.out.gz").write_bytes(gzip.compress((d / "D.out").read_bytes(), mtime=0))
+    if (d / "eigenvector.out").exists():
+        shutil.copyfile(d / "eigenvector.out", OUT / f"refgpu_{name}_eigenvector.out")
+    (OUT / f"refgpu_{name}_stdout.txt").write_text((d / "stdout.txt").read_text())
+
+
 def min_progress(stdout):
     """The minimizer's progress lines of a gpumd / b200md stdout."""
     return [ln for ln in stdout.splitlines() if ln.startswith(("    step ", "    Position step", "  Converged!"))]
@@ -102,10 +178,12 @@ def write_model(path, s, symbols, vel=None):
 ONLY = None  # --only REGEX: run just the matching cases
 
 
-def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1, model_file=None, head=""):
+def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1, model_file=None, head="",
+             files=None):
     """gpus > 1: that many visible devices -> the reference takes its NEP_MULTIGPU path
     (src/force/force.cu:139-160); skipped when the box has fewer.  model_file: copy this model.xyz
-    instead of writing one from s.  head: keywords before the `potential` line (replicate)."""
+    instead of writing one from s.  head: keywords before the `potential` line (replicate).  files: name ->
+    text of further input files (kpoints.in)."""
     if ONLY and not re.search(ONLY, name):
         return None, None
     import os
@@ -129,6 +207,8 @@ def run_case(name, s, symbols, potential, run_in, vel=None, timeout=900, gpus=1,
     else:
         shutil.copyfile(model_file, d / "model.xyz")
     (d / "run.in").write_text(head + "potential potential.txt\n" + run_in)
+    for fname, text in (files or {}).items():
+        (d / fname).write_text(text)
     t0 = time.time()
     r = subprocess.run([str(BIN)], cwd=d, capture_output=True, text=True, timeout=timeout, env=env)
     wall = time.time() - t0
@@ -181,6 +261,14 @@ def main():
         s = make() if make else None
         d, i = run_case(name, s, sym, GOLDEN / pot, lines + MIN_TAIL, model_file=model_file, head=head)
         collect_minimize(d, name); infos.append(i)
+
+    # ---- (0b) phonons ----
+    for name, (make, symbols, pot, head, lines, model_file, kpoints, keep_d) in PHONON_CASES.items():
+        sym = symbols or nep_type_order(GOLDEN / pot)
+        s = make() if make else None
+        d, i = run_case(name, s, sym, GOLDEN / pot, lines, model_file=model_file, head=head,
+                        files={"kpoints.in": kpoints})
+        collect_phonon(d, name, keep_d); infos.append(i)
 
     # ---- (1) single points on the large-box path ----
     pbte_sym = nep_type_order(GOLDEN / "nep_PbTe.txt")
