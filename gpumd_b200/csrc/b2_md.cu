@@ -8,6 +8,7 @@
 #include "b2_lj.cuh"
 #include "b2_neighbor_host.h"
 #include "b2_nep.cuh" // b2_body_unpack
+#include "b2_reduce.cuh"
 #include <cmath>
 #include <cstddef>
 #include <cstdio>
@@ -163,8 +164,7 @@ __global__ void __launch_bounds__(BLK) k_scale_by(
 
 // One pass over mass / velocity / potential / 6 virial rows for all 8 outputs (the reference
 // launches <<<8,1024>>>, one block per output, each striding over all atoms:
-// ensemble.cu:434-633,655).  Warp-shuffle tree -> per-block partials in `scratch` -> the last
-// block to finish (ticket) sums the partials in a fixed order, so the result is deterministic.
+// ensemble.cu:434-633,655), reduced in the fixed order of b2_reduce.cuh: deterministic.
 __global__ void __launch_bounds__(THERMO_BLK) k_thermo(
   int n, int stride, int n_temperature, double volume, const double* __restrict__ mass,
   const double* __restrict__ pe, const double* __restrict__ vel, const double* __restrict__ virial,
@@ -178,59 +178,13 @@ __global__ void __launch_bounds__(THERMO_BLK) k_thermo(
     for (int k = 0; k < 8; ++k)
       s[k] += t[k];
   }
-  __shared__ double red[8][THERMO_BLK / 32];
-  __shared__ bool last;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    double v = s[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0)
-      red[k][wid] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 8) {
-    double v = 0.0;
-    for (int w = 0; w < THERMO_BLK / 32; ++w)
-      v += red[threadIdx.x][w];
-    partial[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = v;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0)
-    last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-  __syncthreads();
-  if (!last)
+  b2_block_totals<8, THERMO_BLK>(s, partial + blockIdx.x, gridDim.x);
+  if (!b2_last_block(ticket))
     return;
-  __threadfence();
-  // final: warp k sums partial row k in a fixed (block-index) order
-  if (wid < 8) {
-    double v = 0.0;
-    for (int b = lane; b < (int)gridDim.x; b += 32)
-      v += partial[(size_t)wid * gridDim.x + b];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0) {
-      const double K_B = 8.617343e-5; // src/utilities/common.cuh:21
-      if (wid == 0)
-        thermo[0] = v / (3.0 * n_temperature * K_B);
-      else if (wid == 1)
-        thermo[1] = v;
-      else
-        thermo[wid] = v / volume;
-    }
-  }
-  if (threadIdx.x == 0)
-    *ticket = 0; // re-arm for the next call on this stream
-}
-
-int thermo_blocks(int n)
-{
-  int g = grid_for(n, THERMO_BLK);
-  return g > THERMO_MAX_BLOCKS ? THERMO_MAX_BLOCKS : (g < 1 ? 1 : g);
+  b2_grid_totals<8, THERMO_BLK>(partial, [&](int k, double v) {
+    const double K_B = 8.617343e-5; // src/utilities/common.cuh:21
+    thermo[k] = k == 0 ? v / (3.0 * n_temperature * K_B) : (k == 1 ? v : v / volume);
+  });
 }
 
 } // namespace
@@ -502,7 +456,7 @@ int b200md_halo_pack(
 
 long long b200md_thermo_scratch_bytes(int n)
 {
-  return (long long)sizeof(double) * 8 * thermo_blocks(n) + 64;
+  return (long long)b2_scratch_bytes(8, b2_reduce_blocks(n, THERMO_BLK, THERMO_MAX_BLOCKS));
 }
 
 int b200md_find_thermo(
@@ -520,13 +474,9 @@ int b200md_find_thermo_strided(
   const double* d_potential, const double* d_velocity, const double* d_virial, double* d_thermo8,
   void* d_scratch, void* stream)
 {
-  // scratch layout: [ticket (64 bytes, must be zero before the FIRST call)] [8*blocks doubles]
-  unsigned int* ticket = (unsigned int*)d_scratch;
-  double* partial = (double*)((char*)d_scratch + 64);
-  const int g = thermo_blocks(n);
-  k_thermo<<<g, THERMO_BLK, 0, (cudaStream_t)stream>>>(
-    n, stride, n_temperature, volume, d_mass, d_potential, d_velocity, d_virial, d_thermo8, partial,
-    ticket);
+  k_thermo<<<b2_reduce_blocks(n, THERMO_BLK, THERMO_MAX_BLOCKS), THERMO_BLK, 0, (cudaStream_t)stream>>>(
+    n, stride, n_temperature, volume, d_mass, d_potential, d_velocity, d_virial, d_thermo8,
+    b2_scratch_partials(d_scratch), b2_scratch_ticket(d_scratch));
   B2_LAUNCHED();
   return B200MD_OK;
 }

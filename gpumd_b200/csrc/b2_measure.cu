@@ -19,6 +19,7 @@
 // Every reduction has a fixed order: the results do not depend on scheduling.
 #include "../../include/b200md.h"
 #include "b2_host.h"
+#include "b2_reduce.cuh"
 #include "b2_tersoff.cuh" // b2_heat5
 #include <cmath>
 #include <new>
@@ -29,59 +30,7 @@ namespace {
 
 constexpr int RED_BLK = 256;        // atoms-per-block of the ticketed reductions
 constexpr int RED_MAX_BLOCKS = 264; // two per SM of an H100 SXM
-
-int red_blocks(int n)
-{
-  const int g = grid_for(n, RED_BLK);
-  return g > RED_MAX_BLOCKS ? RED_MAX_BLOCKS : (g < 1 ? 1 : g);
-}
-
-// Sums s[k] over the block into partial[k * gridDim.x + blockIdx.x].  Returns true in the one block
-// that finishes last (ticket); partial is then complete and visible to it.
-template <int K>
-__device__ bool block_partials(const double (&s)[K], double* partial, unsigned int* ticket)
-{
-  __shared__ double red[K][RED_BLK / 32];
-  __shared__ bool last;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double v = s[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0)
-      red[k][wid] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < K) {
-    double v = 0.0;
-    for (int w = 0; w < RED_BLK / 32; ++w)
-      v += red[threadIdx.x][w];
-    partial[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = v;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0)
-    last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-  __syncthreads();
-  if (last)
-    __threadfence();
-  return last;
-}
-
-// in the last block: warp k < K sums partial row k in block-index order; lane 0 gets the total
-__device__ double final_row(const double* partial, int k)
-{
-  const int lane = threadIdx.x & 31;
-  double v = 0.0;
-  for (int b = lane; b < (int)gridDim.x; b += 32)
-    v += partial[(size_t)k * gridDim.x + b];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1)
-    v += __shfl_down_sync(0xffffffffu, v, o);
-  return v;
-}
+constexpr int FTOT_SLOT = 8;        // doubles of the drive's scratch between the ticket and the partials
 
 // f_i += W_i^T fe, with the virial index map xx xy xz / yx yy yz / zx zy zz = 0 3 4 / 6 1 5 / 7 8 2
 // (force.cu:857-878), and the total of the new forces.  nvcc -O3 compiles force.cu:248-250 to
@@ -106,16 +55,9 @@ __global__ void __launch_bounds__(RED_BLK) k_hnemd_drive(
     t[1] += fy;
     t[2] += fz;
   }
-  if (!block_partials<3>(t, partial, ticket))
-    return;
-  const int wid = threadIdx.x >> 5;
-  if (wid < 3) {
-    const double v = final_row(partial, wid);
-    if ((threadIdx.x & 31) == 0)
-      ftot[wid] = v;
-  }
-  if (threadIdx.x == 0)
-    *ticket = 0; // re-arm for the next call on this stream
+  b2_block_totals<3, RED_BLK>(t, partial + blockIdx.x, gridDim.x);
+  if (b2_last_block(ticket))
+    b2_grid_totals<3, RED_BLK>(partial, [&](int k, double v) { ftot[k] = v; });
 }
 
 // f_i -= ftot / N as gpu_correct_force (force.cu:303-312): a product with the host's 1.0 / N, then
@@ -146,16 +88,9 @@ __global__ void __launch_bounds__(RED_BLK) k_hnemd_heat(
     for (int k = 0; k < 5; ++k)
       t[k] += h[k];
   }
-  if (!block_partials<5>(t, partial, ticket))
-    return;
-  const int wid = threadIdx.x >> 5;
-  if (wid < 5) {
-    const double s = final_row(partial, wid);
-    if ((threadIdx.x & 31) == 0)
-      row5[wid] = s;
-  }
-  if (threadIdx.x == 0)
-    *ticket = 0;
+  b2_block_totals<5, RED_BLK>(t, partial + blockIdx.x, gridDim.x);
+  if (b2_last_block(ticket))
+    b2_grid_totals<5, RED_BLK>(partial, [&](int k, double v) { row5[k] = v; });
 }
 
 // one block per heat component: strided partial sums, then a tree -- the order of hac.cu:50-78
@@ -219,7 +154,7 @@ struct b200md_hnemd {
   int output_interval = 1;
   double fe[3] = {0, 0, 0}, fe_norm = 0.0;
   DevBuf<double> heat_all; // [output_interval][5], row = step % output_interval
-  DevBuf<char> scratch;    // [ticket (64 bytes)][5 * red_blocks(n) partials]
+  DevBuf<char> scratch;    // b2_scratch_bytes(5, blocks of k_hnemd_heat)
 };
 
 extern "C" {
@@ -309,7 +244,7 @@ int b200md_hac_series(b200md_hac* p, double* out, void* stream)
 
 long long b200md_hnemd_drive_scratch_bytes(int n)
 {
-  return 128 + (long long)sizeof(double) * 3 * red_blocks(n);
+  return (long long)(b2_scratch_bytes(3, b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS)) + sizeof(double) * FTOT_SLOT);
 }
 
 int b200md_hnemd_drive(
@@ -320,13 +255,11 @@ int b200md_hnemd_drive(
     set_error("b200md_hnemd_drive: bad argument");
     return B200MD_ERR_ARG;
   }
-  // scratch: [ticket, zero before the FIRST call][ftot[3] at +64][3 * blocks partials at +128]
-  unsigned int* ticket = (unsigned int*)d_scratch;
-  double* ftot = (double*)((char*)d_scratch + 64);
-  double* partial = (double*)((char*)d_scratch + 128);
+  // the b2_scratch_* layout with ftot[3] in front of the partials
+  double* ftot = b2_scratch_partials(d_scratch);
   cudaStream_t st = (cudaStream_t)stream;
-  k_hnemd_drive<<<red_blocks(n), RED_BLK, 0, st>>>(
-    n, stride, fe[0], fe[1], fe[2], d_virial, d_force, partial, ticket, ftot);
+  k_hnemd_drive<<<b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS), RED_BLK, 0, st>>>(
+    n, stride, fe[0], fe[1], fe[2], d_virial, d_force, ftot + FTOT_SLOT, b2_scratch_ticket(d_scratch), ftot);
   B2_LAUNCHED();
   k_hnemd_correct<<<grid_for(n, 256), 256, 0, st>>>(n, stride, 1.0 / n, ftot, d_force);
   B2_LAUNCHED();
@@ -371,15 +304,16 @@ int b200md_hnemd_sample(
     set_error("b200md_hnemd_sample: bad argument");
     return B200MD_ERR_ARG;
   }
-  const size_t need = 64 + sizeof(double) * 5 * red_blocks(n);
+  const int g = b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS);
+  const size_t need = b2_scratch_bytes(5, g);
   if (p->scratch.n < need) { // first call, or more atoms than before: the ticket starts at zero
     B2_CUDA(p->scratch.reserve(need));
-    B2_CUDA(cudaMemsetAsync(p->scratch.p, 0, 64, (cudaStream_t)stream));
+    B2_CUDA(cudaMemsetAsync(p->scratch.p, 0, B2_TICKET_BYTES, (cudaStream_t)stream));
   }
   const int row = step % p->output_interval;
-  k_hnemd_heat<<<red_blocks(n), RED_BLK, 0, (cudaStream_t)stream>>>(
-    n, stride, d_virial, d_velocity, p->heat_all.p + (size_t)5 * row, (double*)(p->scratch.p + 64),
-    (unsigned int*)p->scratch.p);
+  k_hnemd_heat<<<g, RED_BLK, 0, (cudaStream_t)stream>>>(
+    n, stride, d_virial, d_velocity, p->heat_all.p + (size_t)5 * row, b2_scratch_partials(p->scratch.p),
+    b2_scratch_ticket(p->scratch.p));
   B2_LAUNCHED();
   return B200MD_OK;
 }

@@ -15,7 +15,7 @@
 // run-to-run identical on any device.
 #include "../../include/b200md.h"
 #include "b2_host.h"
-#include <algorithm>
+#include "b2_reduce.cuh"
 #include <cmath>
 #include <new>
 
@@ -33,70 +33,6 @@ constexpr double DT_MAX = 10.0 * DT_0, DT_MIN = 0.02 * DT_0;
 constexpr int N_MIN = 20;
 constexpr double STRESS_TOLERANCE_GPA = 1e-4;    // minimizer_fire_box_change.cu:254
 constexpr double SD_DECREASE = 0.2, SD_INCREASE = 1.2; // minimizer_sd.cu:27-28
-
-int red_grid(int n) { return std::min(grid_for(n, BLK), RED_GRID); }
-
-__device__ bool last_block(unsigned int* ticket)
-{
-  __shared__ bool last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0)
-    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last)
-    __threadfence();
-  return last;
-}
-
-// t[0] is a maximum, t[1..K-1] are sums: block result -> partial[blockIdx.x * K + k]
-template <int K>
-__device__ void block_partials(double (&t)[K], double* partial)
-{
-  __shared__ double sm[K][BLK / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double v = t[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double w = __shfl_down_sync(0xffffffffu, v, o);
-      v = k == 0 ? fmax(v, w) : v + w;
-    }
-    if (lane == 0)
-      sm[k][wid] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < K) {
-    const int k = threadIdx.x;
-    double v = sm[k][0];
-    for (int w = 1; w < BLK / 32; ++w)
-      v = k == 0 ? fmax(v, sm[k][w]) : v + sm[k][w];
-    partial[(size_t)blockIdx.x * K + k] = v;
-  }
-}
-
-// in the last block: s[k] = the partials of all blocks combined in block order (one warp per k)
-template <int K>
-__device__ void grid_totals(const double* partial, double* s)
-{
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (int k = wid; k < K; k += BLK / 32) {
-    double v = 0.0; // F^2 >= 0: a neutral start for the maximum too
-    for (int b = lane; b < (int)gridDim.x; b += 32) {
-      const double p = partial[(size_t)b * K + k];
-      v = k == 0 ? fmax(v, p) : v + p;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double w = __shfl_down_sync(0xffffffffu, v, o);
-      v = k == 0 ? fmax(v, w) : v + w;
-    }
-    if (lane == 0)
-      s[k] = v;
-  }
-  __syncthreads();
-}
 
 struct FireParams {
   double tol, volume, L;
@@ -222,15 +158,13 @@ __global__ void __launch_bounds__(BLK) k_fire_reduce(
         t[5 + k] += w[vmap[k] * N + i];
     }
   }
-  block_partials<K>(t, partial);
-  if (!last_block(ticket))
+  b2_block_totals<K, BLK, 1u>(t, partial + blockIdx.x, gridDim.x); // row 0: max F^2
+  if (!b2_last_block(ticket))
     return;
   __shared__ double s[RED_K];
-  grid_totals<K>(partial, s);
-  if (threadIdx.x == 0) {
+  b2_grid_totals<K, BLK, 1u>(partial, [&](int k, double v) { s[k] = v; });
+  if (threadIdx.x == 0)
     fire_control(s, rec, prm);
-    *ticket = 0u;
-  }
 }
 
 // FIRE update per atom (minimizer_fire.cu:148-176, minimizer_fire_box_change.cu:339-403) in the reference's
@@ -280,22 +214,21 @@ __global__ void __launch_bounds__(BLK) k_fire_update(
 __global__ void __launch_bounds__(BLK) k_sd_energy(
   int n, const double* __restrict__ u_trial, double* partial, unsigned int* ticket, double* rec)
 {
-  double t[2] = {0.0, 0.0};
+  double t[1] = {0.0};
   for (int i = blockIdx.x * BLK + threadIdx.x; i < n; i += gridDim.x * BLK)
-    t[1] += u_trial[i];
-  block_partials<2>(t, partial);
-  if (!last_block(ticket))
+    t[0] += u_trial[i];
+  b2_block_totals<1, BLK>(t, partial + blockIdx.x, gridDim.x);
+  if (!b2_last_block(ticket))
     return;
-  __shared__ double s[2];
-  grid_totals<2>(partial, s);
+  __shared__ double Ut;
+  b2_grid_totals<1, BLK>(partial, [&](int, double v) { Ut = v; });
   if (threadIdx.x == 0) {
-    const double U = rec[B200MD_MIN_U], Ut = s[1];
+    const double U = rec[B200MD_MIN_U];
     const bool uphill = Ut > U;
     rec[B200MD_MIN_UTRIAL] = Ut;
     rec[B200MD_MIN_USMALLER] = uphill ? U : Ut;
     rec[B200MD_MIN_UPHILL] = uphill ? 1.0 : 0.0;
     rec[B200MD_MIN_STEP] *= uphill ? SD_DECREASE : SD_INCREASE;
-    *ticket = 0u;
   }
 }
 
@@ -331,18 +264,17 @@ __global__ void __launch_bounds__(BLK) k_sd_accept(
     }
     t[1] += ui;
   }
-  block_partials<2>(t, partial);
-  if (!last_block(ticket))
+  b2_block_totals<2, BLK, 1u>(t, partial + blockIdx.x, gridDim.x); // row 0: max F^2
+  if (!b2_last_block(ticket))
     return;
   __shared__ double s[2];
-  grid_totals<2>(partial, s);
+  b2_grid_totals<2, BLK, 1u>(partial, [&](int k, double v) { s[k] = v; });
   if (threadIdx.x == 0) {
     const double f_max = sqrt(s[0]);
     rec[B200MD_MIN_FMAX] = f_max;
     rec[B200MD_MIN_U] = s[1];
     rec[B200MD_MIN_CONVERGED] = f_max < tol ? 1.0 : 0.0;
     rec[B200MD_MIN_SCALE] = rec[B200MD_MIN_STEP] / f_max;
-    *ticket = 0u;
   }
 }
 
@@ -500,7 +432,7 @@ int b200md_minimizer_sd_begin(
       bad_sd(d_position_trial, d_force_trial, d_potential_trial, fixed_group, d_group_label))
     return B200MD_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  k_sd_accept<<<red_grid(n), BLK, 0, st>>>(
+  k_sd_accept<<<b2_reduce_blocks(n, BLK, RED_GRID), BLK, 0, st>>>(
     n, 1, d_position, d_force, d_potential, d_position_trial, d_force_trial, d_potential_trial, p->partial.p, p->ticket.p, p->rec.p,
     p->tol);
   B2_LAUNCHED();
@@ -516,7 +448,7 @@ int b200md_minimizer_sd_step(
       bad_sd(d_position_trial, d_force_trial, d_potential_trial, fixed_group, d_group_label))
     return B200MD_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  const int g = red_grid(n);
+  const int g = b2_reduce_blocks(n, BLK, RED_GRID);
   k_sd_energy<<<g, BLK, 0, st>>>(n, d_potential_trial, p->partial.p, p->ticket.p, p->rec.p);
   B2_LAUNCHED();
   k_sd_accept<<<g, BLK, 0, st>>>(
@@ -544,12 +476,12 @@ int b200md_minimizer_fire_step(
     if (!(p->L > 0.0)) // L = cbrt(V) of the box the minimization starts from
       p->L = std::cbrt(prm.volume);
     prm.L = p->L;
-    k_fire_reduce<true><<<red_grid(n), BLK, 0, st>>>(
+    k_fire_reduce<true><<<b2_reduce_blocks(n, BLK, RED_GRID), BLK, 0, st>>>(
       n, d_force, p->v.p, d_potential, d_virial, p->partial.p, p->ticket.p, p->rec.p, prm);
     B2_LAUNCHED();
     k_fire_update<true><<<grid_for(n, BLK), BLK, 0, st>>>(n, d_position, p->v.p, d_force, p->rec.p);
   } else {
-    k_fire_reduce<false><<<red_grid(n), BLK, 0, st>>>(
+    k_fire_reduce<false><<<b2_reduce_blocks(n, BLK, RED_GRID), BLK, 0, st>>>(
       n, d_force, p->v.p, d_potential, nullptr, p->partial.p, p->ticket.p, p->rec.p, prm);
     B2_LAUNCHED();
     k_fire_update<false><<<grid_for(n, BLK), BLK, 0, st>>>(n, d_position, p->v.p, d_force, p->rec.p);

@@ -17,6 +17,7 @@
 #include "b2_bdp.cuh"
 #include "b2_host.h"
 #include "b2_integrate.cuh"
+#include "b2_reduce.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstddef>
@@ -38,37 +39,6 @@ struct HeatState {
   double factor[2];    // scale factors of the last rescaling
   double energy[2];    // energy transferred from the system to the source / sink baths (eV)
 };
-
-// sum of t[0..K-1] over the block into s[0..K-1] (warp shuffles, then one warp over the warps)
-template <int K>
-__device__ void block_sum(double (&t)[K], double (*sm)[BLK / 32])
-{
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double v = t[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0)
-      sm[k][wid] = v;
-  }
-  __syncthreads();
-}
-
-// last-block ticket: true in every thread of the block that finished last
-__device__ bool last_block(unsigned int* ticket)
-{
-  __shared__ bool last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0)
-    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last)
-    __threadfence();
-  return last;
-}
 
 __global__ void __launch_bounds__(BLK) k_heat_init_states(
   curandState* state, int n_source, int n_total, unsigned long long seed_source,
@@ -109,29 +79,9 @@ __global__ void __launch_bounds__(BLK) k_heat_lan(
     g_state[m] = state;
     t[g] = 0.5 * ms * de;
   }
-  __shared__ double sm[2][BLK / 32];
-  block_sum<2>(t, sm);
-  if (threadIdx.x < 2) {
-    double v = 0.0;
-    for (int w = 0; w < BLK / 32; ++w)
-      v += sm[threadIdx.x][w];
-    partial[(size_t)blockIdx.x * 2 + threadIdx.x] = v;
-  }
-  if (!last_block(ticket))
-    return;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (wid < 2) { // fixed order over the blocks
-    double v = 0.0;
-    for (int b = lane; b < (int)gridDim.x; b += 32)
-      v += partial[(size_t)b * 2 + wid];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0)
-      hs->energy[wid] += v;
-  }
-  if (threadIdx.x == 0)
-    *ticket = 0u;
+  b2_block_totals<2, BLK>(t, partial + blockIdx.x, gridDim.x);
+  if (b2_last_block(ticket))
+    b2_grid_totals<2, BLK>(partial, [&](int g, double v) { hs->energy[g] += v; });
 }
 
 // the serial bodies of the reduction tail, kept out of line so that they do not set the register
@@ -172,33 +122,13 @@ __global__ void __launch_bounds__(BLK) k_heat_reduce(
         t[k + 4] = (vx * vx + vy * vy + vz * vz) * ms;
       }
   }
-  __shared__ double sm[10][BLK / 32];
-  block_sum<10>(t, sm);
-  if (threadIdx.x < 10) {
-    double v = 0.0;
-    for (int w = 0; w < BLK / 32; ++w)
-      v += sm[threadIdx.x][w];
-    partial[(size_t)blockIdx.x * 10 + threadIdx.x] = v;
-  }
-  if (!last_block(ticket))
+  b2_block_totals<10, BLK>(t, partial + blockIdx.x, gridDim.x);
+  if (!b2_last_block(ticket))
     return;
   __shared__ double tot[10];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (int k = wid; k < 10; k += BLK / 32) {
-    double v = 0.0;
-    for (int b = lane; b < (int)gridDim.x; b += 32)
-      v += partial[(size_t)b * 10 + k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0)
-      tot[k] = v;
-  }
-  __syncthreads();
+  b2_grid_totals<10, BLK>(partial, [&](int k, double v) { tot[k] = v; });
   if (threadIdx.x >= 2)
     return;
-  if (threadIdx.x == 0)
-    *ticket = 0u;
   double ek2[2];
   const int size[2] = {n_source, n_total - n_source};
   for (int g = 0; g < 2; ++g) {
@@ -258,7 +188,7 @@ constexpr int NQ = 23;
 __constant__ int c_virial_row[9] = {0, 3, 4, 6, 1, 5, 7, 8, 2};
 
 // Segmented reduction: the group contents are cut into chunks of at most CHUNK entries, and each
-// (chunk, group) overlap is one segment that one block reduces into partial[segment][NQ].  Many
+// (chunk, group) overlap is one segment that one block reduces into partial[q][segment].  Many
 // small groups give many short segments, one large group many full ones: all SMs stay busy either
 // way, and empty groups have no segment.
 constexpr int CHUNK = 4 * BLK;
@@ -326,33 +256,21 @@ __global__ void __launch_bounds__(BLK) k_group_partial(
       t[22] += vz * m;
     }
   }
-  __shared__ double sm[NQ][BLK / 32];
-  block_sum<NQ>(t, sm);
-  if (threadIdx.x < NQ) {
-    double v = 0.0;
-    for (int w = 0; w < BLK / 32; ++w)
-      v += sm[threadIdx.x][w];
-    partial[(size_t)s * NQ + threadIdx.x] = v;
-  }
+  b2_block_totals<NQ, BLK>(t, partial + s, gridDim.x);
 }
 
 // one warp per (column, group): the group's segments in order, added to the running sum
 __global__ void __launch_bounds__(BLK) k_group_finish(
-  int num_groups, int num_cols, const int* __restrict__ col_q, const int* __restrict__ group_seg,
-  const double* __restrict__ partial, double* sum)
+  int num_groups, int num_cols, int num_segments, const int* __restrict__ col_q,
+  const int* __restrict__ group_seg, const double* __restrict__ partial, double* sum)
 {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (warp >= num_groups * num_cols)
     return;
   const int c = warp / num_groups, g = warp - c * num_groups;
-  const int q = col_q[c];
-  double v = 0.0;
-  for (int s = group_seg[g] + lane; s < group_seg[g + 1]; s += 32)
-    v += partial[(size_t)s * NQ + q];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1)
-    v += __shfl_down_sync(0xffffffffu, v, o);
-  if (lane == 0)
+  const double v = b2_warp_ordered(
+    partial + (size_t)col_q[c] * num_segments + group_seg[g], group_seg[g + 1] - group_seg[g]);
+  if ((threadIdx.x & 31) == 0)
     sum[warp] += v; // column-major blocks of num_groups, as gpu_group_sum
 }
 
@@ -669,7 +587,7 @@ int b200md_group_compute_sample(
   }
   const long long threads = 32LL * p->num_cols * p->num_groups;
   k_group_finish<<<grid_for(threads, BLK), BLK, 0, st>>>(
-    p->num_groups, p->num_cols, p->col_q.p, p->group_seg.p, p->partial.p, p->sum.p);
+    p->num_groups, p->num_cols, p->num_segments, p->col_q.p, p->group_seg.p, p->partial.p, p->sum.p);
   B2_LAUNCHED();
   return B200MD_OK;
 }

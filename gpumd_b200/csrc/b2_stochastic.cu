@@ -12,10 +12,11 @@
 // The per-atom generator is cuRAND's XORWOW exactly as the reference uses it -- curand_init(seed, n, 0)
 // and three curand_normal_double draws per atom per call -- so a run seeded like the reference
 // (its -DDEBUG build passes glibc's first rand() = 1804289383) follows the reference's noise stream
-// draw for draw.  The momentum sums are one fused deterministic reduction (warp shuffles, per-block
-// partials, last-block ticket) instead of the reference's <<<4,1024>>> strided loops.
+// draw for draw.  The momentum sums are one fused deterministic reduction (the block stage and ticket
+// of b2_reduce.cuh) instead of the reference's <<<4,1024>>> strided loops.
 #include "../../include/b200md.h"
 #include "b2_host.h"
+#include "b2_reduce.cuh"
 #include <cmath>
 #include <curand_kernel.h>
 #include <new>
@@ -53,37 +54,13 @@ __global__ void __launch_bounds__(BLK) k_langevin(
     t[3] = m;
     g_state[i] = state;
   }
-  __shared__ double sm[BLK / 32][4];
-  __shared__ bool last;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    double v = t[k];
-    for (int o = 16; o > 0; o >>= 1)
-      v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0)
-      sm[threadIdx.x >> 5][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 4) {
+  b2_block_totals<4, BLK>(t, partial + blockIdx.x, gridDim.x);
+  // the blocks in index order by one thread per row (the order of b2_grid_totals differs)
+  if (b2_last_block(ticket) && threadIdx.x < 4) {
     double v = 0.0;
-    for (int w = 0; w < BLK / 32; ++w)
-      v += sm[w][threadIdx.x];
-    partial[(size_t)blockIdx.x * 4 + threadIdx.x] = v;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0)
-    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last) { // fixed summation order over the blocks: run-to-run deterministic
-    if (threadIdx.x < 4) {
-      double v = 0.0;
-      for (unsigned b = 0; b < gridDim.x; ++b)
-        v += partial[(size_t)b * 4 + threadIdx.x];
-      mom4[threadIdx.x] = v;
-    }
-    if (threadIdx.x == 0)
-      *ticket = 0u;
+    for (unsigned b = 0; b < gridDim.x; ++b)
+      v += partial[(size_t)threadIdx.x * gridDim.x + b];
+    mom4[threadIdx.x] = v;
   }
 }
 
