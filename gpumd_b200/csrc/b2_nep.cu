@@ -25,6 +25,17 @@ constexpr int MLP_BLK = 256;
 // blocks fit an SM's 228 KB of shared memory (1 KB reserved per block)
 constexpr int FUSED_DIMP = 32;
 constexpr size_t FUSED_MAX_SMEM = 113 * 1024;
+// Angular shapes k_angular_fused is compiled for (B2AngShape): NEP4's default n_max = 4 4 with l_max = 4 2 0
+// (dim 30) and 4 0 0 (dim 25).  Each shape adds 12 instances (NT x K1 x ORTHO, about 15 s of build time);
+// every other shape within the budget runs the run-time-shape instance.
+enum { FUSED_SHAPE_NONE, FUSED_SHAPE_RT, FUSED_SHAPE_4B, FUSED_SHAPE_3B };
+
+int fused_shape_of(const NepModel& m)
+{
+  if (m.nr1 == 5 && m.na1 == 5 && !m.has1111)
+    return m.has222 ? FUSED_SHAPE_4B : FUSED_SHAPE_3B;
+  return FUSED_SHAPE_RT;
+}
 
 __global__ void __launch_bounds__(BLK) k_split(B2NepView P, B2Box box)
 {
@@ -388,6 +399,7 @@ struct b200md_nep {
   bool fuse_split = false; // many-type path: neighbour split inside the radial descriptor pass
   bool use_tc = false; // hidden layer on the tensor cores (k_mlp_tc) instead of k_mlp
   bool ang_fused = false; // k_angular_fused instead of k_desc_angular2 + hidden layer + k_force_angular2
+  int fused_shape = 0;     // its instance: FUSED_SHAPE_* (b200md_nep_info 10)
   size_t fused_smem = 0;  // its dynamic shared memory per block
   bool slot_map = false;  // k_force_final2: thread per tile slot (type-pure warps); measured slower
                           // (H100, 1 M-atom PbTe: 1.26 vs 1.02 ms), B200MD_NEP_SLOTMAP=1 for A/B runs
@@ -637,10 +649,10 @@ int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool 
   return B200MD_OK;
 }
 
-template <int NT, int K1, int DIMP, bool ORTHO>
+template <int NT, int K1, int DIMP, bool ORTHO, class SH>
 int launch_fused_inst(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
-  auto kern = k_angular_fused<NT, K1, DIMP, ORTHO>;
+  auto kern = k_angular_fused<NT, K1, DIMP, ORTHO, SH>;
   if (p->fused_smem > 48 * 1024)
     B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->fused_smem));
   kern<<<grid_for(p->n, BLK), BLK, p->fused_smem, st>>>(
@@ -649,15 +661,26 @@ int launch_fused_inst(const b200md_nep* p, const B2Box& box, cudaStream_t st)
   return B200MD_OK;
 }
 
-// the one hidden-layer width k_angular_fused is instantiated for (FUSED_DIMP, see nep_setup)
+template <int K1, class SH>
+int launch_fused_shape(const b200md_nep* p, const B2Box& box, cudaStream_t st)
+{
+  if (p->model.nt == 1)
+    return box.ortho ? launch_fused_inst<1, K1, FUSED_DIMP, true, SH>(p, box, st)
+                     : launch_fused_inst<1, K1, FUSED_DIMP, false, SH>(p, box, st);
+  return box.ortho ? launch_fused_inst<2, K1, FUSED_DIMP, true, SH>(p, box, st)
+                   : launch_fused_inst<2, K1, FUSED_DIMP, false, SH>(p, box, st);
+}
+
+// the one hidden-layer width k_angular_fused is instantiated for (FUSED_DIMP, see nep_setup), on the angular
+// shape p->fused_shape (fused_shape_of)
 template <int K1>
 int launch_angular_fused(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
-  if (p->model.nt == 1)
-    return box.ortho ? launch_fused_inst<1, K1, FUSED_DIMP, true>(p, box, st)
-                     : launch_fused_inst<1, K1, FUSED_DIMP, false>(p, box, st);
-  return box.ortho ? launch_fused_inst<2, K1, FUSED_DIMP, true>(p, box, st)
-                   : launch_fused_inst<2, K1, FUSED_DIMP, false>(p, box, st);
+  switch (p->fused_shape) {
+    case FUSED_SHAPE_4B: return launch_fused_shape<K1, B2AngShape<5, 5, true, false>>(p, box, st);
+    case FUSED_SHAPE_3B: return launch_fused_shape<K1, B2AngShape<5, 5, false, false>>(p, box, st);
+    default: return launch_fused_shape<K1, B2AngShapeRT>(p, box, st);
+  }
 }
 
 template <int DIMP>
@@ -846,6 +869,7 @@ int nep_setup(b200md_nep* p, int num_atoms)
   const bool fused_fits = m.nt <= 2 && !mlp_env && m.DIMP == FUSED_DIMP &&
                           p->fused_smem <= FUSED_MAX_SMEM;
   p->ang_fused = fused_fits && p->radial_v2;
+  p->fused_shape = p->ang_fused ? fused_shape_of(m) : FUSED_SHAPE_NONE;
   p->use_tc = m.tc_ok && !mlp_simt && !fused_fits;
   if (p->radial_v2)
     B2_TRY(p->nb.enable_planes());
@@ -1105,6 +1129,7 @@ int b200md_nep_info(const b200md_nep* p, int what)
     case 7: return p->sched ? p->nb.num_segments() : 0;
     case 8: return nep_tile_count(p);
     case 9: return p->tc_ctas_last;
+    case 10: return p->fused_shape;
     default: return -1;
   }
 }

@@ -640,22 +640,24 @@ B2_HD void b2_ang_weights(const float* s, const float* F6, int has222, int has11
       wv[st + k] = 4.0f * F * C3B[st + k] * s[st + k];
     st += 2 * L + 1;
   }
+  // the chain-rule terms are added with explicit FMAs: with has222 / has1111 known at compile time the
+  // compiler could otherwise fuse the product above into the add instead, which rounds differently
   if (has222) {
     const float F = F6[4];
     const float* t = &s[3];
-    wv[3] += F * (3.0f * B2_C4B0 * t[0] * t[0] + B2_C4B1 * (t[1] * t[1] + t[2] * t[2]) +
-                  B2_C4B2 * (t[3] * t[3] + t[4] * t[4]));
-    wv[4] += F * (2.0f * B2_C4B1 * t[0] * t[1] - 2.0f * B2_C4B3 * t[3] * t[1] + B2_C4B4 * t[2] * t[4]);
-    wv[5] += F * (2.0f * B2_C4B1 * t[0] * t[2] + 2.0f * B2_C4B3 * t[3] * t[2] + B2_C4B4 * t[1] * t[4]);
-    wv[6] += F * (2.0f * B2_C4B2 * t[0] * t[3] + B2_C4B3 * (t[2] * t[2] - t[1] * t[1]));
-    wv[7] += F * (2.0f * B2_C4B2 * t[0] * t[4] + B2_C4B4 * t[1] * t[2]);
+    wv[3] = fmaf(F, 3.0f * B2_C4B0 * t[0] * t[0] + B2_C4B1 * (t[1] * t[1] + t[2] * t[2]) +
+                      B2_C4B2 * (t[3] * t[3] + t[4] * t[4]), wv[3]);
+    wv[4] = fmaf(F, 2.0f * B2_C4B1 * t[0] * t[1] - 2.0f * B2_C4B3 * t[3] * t[1] + B2_C4B4 * t[2] * t[4], wv[4]);
+    wv[5] = fmaf(F, 2.0f * B2_C4B1 * t[0] * t[2] + 2.0f * B2_C4B3 * t[3] * t[2] + B2_C4B4 * t[1] * t[4], wv[5]);
+    wv[6] = fmaf(F, 2.0f * B2_C4B2 * t[0] * t[3] + B2_C4B3 * (t[2] * t[2] - t[1] * t[1]), wv[6]);
+    wv[7] = fmaf(F, 2.0f * B2_C4B2 * t[0] * t[4] + B2_C4B4 * t[1] * t[2], wv[7]);
   }
   if (has1111) {
     const float F = F6[5];
     const float tt = s[1] * s[1] + s[2] * s[2];
-    wv[0] += F * (4.0f * B2_C5B0 * s[0] * s[0] * s[0] + 2.0f * B2_C5B1 * tt * s[0]);
-    wv[1] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[1] + 4.0f * B2_C5B2 * tt * s[1]);
-    wv[2] += F * (2.0f * B2_C5B1 * s[0] * s[0] * s[2] + 4.0f * B2_C5B2 * tt * s[2]);
+    wv[0] = fmaf(F, 4.0f * B2_C5B0 * s[0] * s[0] * s[0] + 2.0f * B2_C5B1 * tt * s[0], wv[0]);
+    wv[1] = fmaf(F, 2.0f * B2_C5B1 * s[0] * s[0] * s[1] + 4.0f * B2_C5B2 * tt * s[1], wv[1]);
+    wv[2] = fmaf(F, 2.0f * B2_C5B1 * s[0] * s[0] * s[2] + 4.0f * B2_C5B2 * tt * s[2], wv[2]);
   }
 }
 
@@ -767,6 +769,37 @@ B2_HD void b2_body_desc_angular(
 // multiplied by q_scaler) in Fp[DIMP].  w0 / b0 / w1 are the rows of the atom's type.  Shared by
 // b2_body_mlp and k_angular_fused (b2_nep_angular.cuh), so both produce the same bits.
 template <int DIMP, bool GLOBAL_W>
+B2_HD void b2_mlp_row(const float4* w0, int n, float4* w)
+{
+  const float4* row = w0 + (size_t)n * (DIMP / 4);
+#pragma unroll
+  for (int d = 0; d < DIMP / 4; ++d)
+    w[d] = GLOBAL_W ? B2_LDG(&row[d]) : row[d];
+}
+
+// activation of neuron n from its dot product, then its terms of F and of every Fp[d]
+template <int DIMP, bool GLOBAL_W>
+B2_HD void b2_mlp_neuron(
+  float dot, const float4* w, const float* b0, const float* w1, int n, float& F, float* Fp)
+{
+  const float x1 = tanhf(dot - (GLOBAL_W ? B2_LDG(&b0[n]) : b0[n]));
+  const float w1n = GLOBAL_W ? B2_LDG(&w1[n]) : w1[n];
+  F = fmaf(w1n, x1, F);
+  const float coef = w1n * (1.0f - x1 * x1);
+#pragma unroll
+  for (int d = 0; d < DIMP / 4; ++d) {
+    Fp[4 * d] = fmaf(coef, w[d].x, Fp[4 * d]);
+    Fp[4 * d + 1] = fmaf(coef, w[d].y, Fp[4 * d + 1]);
+    Fp[4 * d + 2] = fmaf(coef, w[d].z, Fp[4 * d + 2]);
+    Fp[4 * d + 3] = fmaf(coef, w[d].w, Fp[4 * d + 3]);
+  }
+}
+
+// PAIR (k_angular_fused on a fixed angular shape, DIMP = 32): the forward dot products of two neurons are formed together, two
+// independent chains of DIMP dependent FMAs in flight instead of one, each still summed in order over d;
+// the activations, F and the Fp updates then follow neuron by neuron in the order n, n+1.  Both forms
+// give the same bits.  k_mlp keeps one chain: at DIMP >= 64 the second row of weights makes it spill.
+template <int DIMP, bool GLOBAL_W, bool PAIR = false>
 B2_HD float b2_mlp_core(
   const float* q, const float4* w0, const float* b0, const float* w1, int nneu, float bias,
   const float* q_scaler, float* Fp)
@@ -775,12 +808,31 @@ B2_HD float b2_mlp_core(
   for (int d = 0; d < DIMP; ++d)
     Fp[d] = 0.0f;
   float F = 0.0f;
-  for (int n = 0; n < nneu; ++n) {
-    const float4* row = w0 + (size_t)n * (DIMP / 4);
-    float4 w[DIMP / 4];
+  int n = 0;
+  if (PAIR) {
+    for (; n + 1 < nneu; n += 2) {
+      float4 wa[DIMP / 4], wb[DIMP / 4];
+      b2_mlp_row<DIMP, GLOBAL_W>(w0, n, wa);
+      b2_mlp_row<DIMP, GLOBAL_W>(w0, n + 1, wb);
+      float da = 0.0f, db = 0.0f;
 #pragma unroll
-    for (int d = 0; d < DIMP / 4; ++d)
-      w[d] = GLOBAL_W ? B2_LDG(&row[d]) : row[d];
+      for (int d = 0; d < DIMP / 4; ++d) {
+        da = fmaf(wa[d].x, q[4 * d], da);
+        db = fmaf(wb[d].x, q[4 * d], db);
+        da = fmaf(wa[d].y, q[4 * d + 1], da);
+        db = fmaf(wb[d].y, q[4 * d + 1], db);
+        da = fmaf(wa[d].z, q[4 * d + 2], da);
+        db = fmaf(wb[d].z, q[4 * d + 2], db);
+        da = fmaf(wa[d].w, q[4 * d + 3], da);
+        db = fmaf(wb[d].w, q[4 * d + 3], db);
+      }
+      b2_mlp_neuron<DIMP, GLOBAL_W>(da, wa, b0, w1, n, F, Fp);
+      b2_mlp_neuron<DIMP, GLOBAL_W>(db, wb, b0, w1, n + 1, F, Fp);
+    }
+  }
+  for (; n < nneu; ++n) {
+    float4 w[DIMP / 4];
+    b2_mlp_row<DIMP, GLOBAL_W>(w0, n, w);
     float dot = 0.0f;
 #pragma unroll
     for (int d = 0; d < DIMP / 4; ++d) {
@@ -789,17 +841,7 @@ B2_HD float b2_mlp_core(
       dot = fmaf(w[d].z, q[4 * d + 2], dot);
       dot = fmaf(w[d].w, q[4 * d + 3], dot);
     }
-    const float x1 = tanhf(dot - (GLOBAL_W ? B2_LDG(&b0[n]) : b0[n]));
-    const float w1n = GLOBAL_W ? B2_LDG(&w1[n]) : w1[n];
-    F = fmaf(w1n, x1, F);
-    const float coef = w1n * (1.0f - x1 * x1);
-#pragma unroll
-    for (int d = 0; d < DIMP / 4; ++d) {
-      Fp[4 * d] = fmaf(coef, w[d].x, Fp[4 * d]);
-      Fp[4 * d + 1] = fmaf(coef, w[d].y, Fp[4 * d + 1]);
-      Fp[4 * d + 2] = fmaf(coef, w[d].z, Fp[4 * d + 2]);
-      Fp[4 * d + 3] = fmaf(coef, w[d].w, Fp[4 * d + 3]);
-    }
+    b2_mlp_neuron<DIMP, GLOBAL_W>(dot, w, b0, w1, n, F, Fp);
   }
   F -= bias;
 #pragma unroll
@@ -859,27 +901,44 @@ B2_HD void b2_body_utable(int i, const B2NepView& P)
   }
 }
 
+// for (n = 0; n < count; n += step) f(n): fully unrolled when FIXED (count is then a compile-time constant,
+// k_angular_fused on a fixed angular shape), otherwise left to the compiler as a run-time loop
+template <bool FIXED, class F>
+B2_HD void b2_channel_loop(int count, int step, F f)
+{
+  if constexpr (FIXED) {
+#pragma unroll
+    for (int n = 0; n < count; n += step)
+      f(n);
+  } else {
+    for (int n = 0; n < count; n += step)
+      f(n);
+  }
+}
+
 // same contraction into the compact planes of the few-type kernels (B2NepView::u_planes == 2):
 // KQ = (K1-1)/4 float4 planes U4[(t2*KQ + q)*n + i] and a float plane [t2*n + i] for k = K1-1.
-// fr(n) = dU/dq[n] of atom i (type t), n < nr1.  Shared by k_utable and k_angular_fused.
-template <int K1, class FpR>
+// fr(n) = dU/dq[n] of atom i (type t), n < nr1.  Shared by k_utable and k_angular_fused.  NR1 > 0: nr1 is
+// that compile-time constant (k_angular_fused on a fixed model shape), so fr is called with constants.
+template <int K1, int NR1 = 0, class FpR>
 B2_HD void b2_utable_compact(const B2NepView& P, int i, int t, FpR fr)
 {
   constexpr int KQ = (K1 - 1) / 4;
+  const int nr1 = NR1 > 0 ? NR1 : P.nr1;
   float4* U4 = reinterpret_cast<float4*>(P.U);
   float* Uf = P.U + (size_t)P.nt * KQ * 4 * P.n;
   for (int t2 = 0; t2 < P.nt; ++t2) {
-    const float* c = P.c_r + (size_t)(t * P.nt + t2) * P.nr1 * K1;
+    const float* c = P.c_r + (size_t)(t * P.nt + t2) * nr1 * K1;
     float u[K1];
 #pragma unroll
     for (int k = 0; k < K1; ++k)
       u[k] = 0.0f;
-    for (int n = 0; n < P.nr1; ++n) {
+    b2_channel_loop<(NR1 > 0)>(nr1, 1, [&](int n) {
       const float f = fr(n);
 #pragma unroll
       for (int k = 0; k < K1; ++k)
         u[k] = fmaf(f, B2_LDG(&c[n * K1 + k]), u[k]);
-    }
+    });
 #pragma unroll
     for (int q = 0; q < KQ; ++q) {
       float4 v;

@@ -26,6 +26,24 @@ namespace b2 {
 
 constexpr int B2_ABC4 = B2_NABC / 4; // float4 groups of one angular channel
 
+// Shape of the angular model: nr1 radial and na1 angular channels, the 4-body (has222) and 5-body
+// (has1111) invariant blocks.  NA1 = 0 reads all four from the model at run time; otherwise they are
+// compile-time constants, so the channel loops unroll and dU/dq is indexed with constants.
+template <int NR1, int NA1, bool H222, bool H1111>
+struct B2AngShape {
+  static constexpr bool fixed = NA1 > 0;
+  static __device__ __forceinline__ int nr1(const B2NepView& P) { return fixed ? NR1 : P.nr1; }
+  static __device__ __forceinline__ int na1(const B2NepView& P) { return fixed ? NA1 : P.na1; }
+  static __device__ __forceinline__ int has222(const B2NepView& P) { return fixed ? H222 : P.has222; }
+  static __device__ __forceinline__ int has1111(const B2NepView& P) { return fixed ? H1111 : P.has1111; }
+  static __device__ __forceinline__ int dim(const B2NepView& P)
+  {
+    return fixed ? NR1 + NA1 * (4 + (H222 ? 1 : 0) + (H1111 ? 1 : 0)) : P.dim;
+  }
+  static constexpr int nr1_const = fixed ? NR1 : 0; // 0: run time (b2_utable_compact)
+};
+using B2AngShapeRT = B2AngShape<0, 0, false, false>;
+
 // angular pair cutoffs of a type-t1 atom against neighbour types 0 .. NT-1, pinned in registers
 template <int NT>
 __device__ __forceinline__ void b2_ang_cutoffs(const B2NepView& P, int t1, float* rc, float* rcinv)
@@ -58,7 +76,7 @@ __device__ __forceinline__ void b2_stage_ctab(const B2NepView& P, float4* dst, i
 // emit_q(k, v): descriptor component k (nr1 <= k < dim); emit_s(g, v): float4 group g = n*6 + abc/4 of
 // the sums s[n][abc].
 // ---------------------------------------------------------------------------------------------
-template <int NT, int K1, int NCH, bool ORTHO, class EmitQ, class EmitS>
+template <int NT, int K1, int NCH, bool ORTHO, class SH, class EmitQ, class EmitS>
 __device__ __forceinline__ void b2_ang_desc_atom(
   const B2NepView& P, const int4* __restrict__ p0, const double* __restrict__ pz, const B2Box& box,
   int i, const B2Rec& a1, const float4* ctab_s, EmitQ emit_q, EmitS emit_s)
@@ -67,7 +85,7 @@ __device__ __forceinline__ void b2_ang_desc_atom(
   constexpr int KQ = (K1 + 3) / 4;
   const B2GeoR geo = b2_geo_pinned(box);
   const unsigned N = (unsigned)P.n;
-  const int na1 = P.na1;
+  const int na1 = SH::na1(P);
   const int t1 = a1.t;
   float rcv[NT], rciv[NT];
   b2_ang_cutoffs<NT>(P, t1, rcv, rciv);
@@ -77,7 +95,7 @@ __device__ __forceinline__ void b2_ang_desc_atom(
     crow[t] = ctab_s + (t1 * P.nt + (t < P.nt ? t : 0)) * na1 * KQ;
   const int* __restrict__ list = P.nl_a;
   const int nn = P.nn_a[i];
-  for (int n0 = 0; n0 < na1; n0 += NCH) {
+  b2_channel_loop<SH::fixed>(na1, NCH, [&](int n0) {
     float s[NCH][B2_NABC];
 #pragma unroll
     for (int c = 0; c < NCH; ++c)
@@ -127,14 +145,14 @@ __device__ __forceinline__ void b2_ang_desc_atom(
     for (int c = 0; c < NCH; ++c) {
       const int n = n0 + c;
       if (n < na1) {
-        b2_ang_invariants(s[c], P.has222, P.has1111,
-                          [&](int blk, float v) { emit_q(P.nr1 + blk * na1 + n, v); });
+        b2_ang_invariants(s[c], SH::has222(P), SH::has1111(P),
+                          [&](int blk, float v) { emit_q(SH::nr1(P) + blk * na1 + n, v); });
 #pragma unroll
         for (int g = 0; g < B2_ABC4; ++g)
           emit_s(n * B2_ABC4 + g, make_float4(s[c][4 * g], s[c][4 * g + 1], s[c][4 * g + 2], s[c][4 * g + 3]));
       }
     }
-  }
+  });
 }
 
 template <int NT, int K1, int NCH, bool ORTHO>
@@ -159,7 +177,7 @@ __global__ void __launch_bounds__(128, 3) k_desc_angular2(
   // in two passes over the list.
   float* const qs = reinterpret_cast<float*>(ctab_s + P.nt * P.nt * P.na1 * KQ) + threadIdx.x;
   float4* __restrict__ sf4 = reinterpret_cast<float4*>(P.sfx);
-  b2_ang_desc_atom<NT, K1, NCH, ORTHO>(
+  b2_ang_desc_atom<NT, K1, NCH, ORTHO, B2AngShapeRT>(
     P, p0, pz, box, i, a1, ctab_s,
     [&](int k, float v) { *(P.qt ? qs + (size_t)(k - P.nr1) * 128 : qb + (size_t)k * N) = v; },
     [&](int g, float4 v) { sf4[(size_t)g * N + i] = v; });
@@ -188,14 +206,14 @@ __host__ __device__ constexpr int b2_ang_ws4(int na1) { return B2_ABC4 * na1 + 1
 
 // The pair loop of sorted atom i (record a1): w = its row of weights dU/ds[n][abc] (float4 group
 // n*6 + abc/4), ctab_s the staged coefficient table.
-template <int NT, int K1, bool ORTHO>
+template <int NT, int K1, bool ORTHO, class SH>
 __device__ __forceinline__ void b2_ang_force_pairs(
   const B2NepView& P, const int4* __restrict__ p0, const double* __restrict__ pz, const B2Box& box,
   int i, const B2Rec& a1, const float4* w, const float4* ctab_s, int* __restrict__ arev)
 {
   constexpr int KQ = (K1 + 3) / 4;
   const unsigned N = (unsigned)P.n;
-  const int na1 = P.na1;
+  const int na1 = SH::na1(P);
   const B2GeoR geo = b2_geo_pinned(box);
   const int t1 = a1.t;
   float rcv[NT], rciv[NT];
@@ -249,7 +267,7 @@ __device__ __forceinline__ void b2_ang_force_pairs(
       Wp[abc] = 0.0f;
     }
     const float4* c4 = ty ? crow[NT - 1] : crow[0];
-    for (int n = 0; n < na1; ++n) {
+    b2_channel_loop<SH::fixed>(na1, 1, [&](int n) {
       float ck[KQ * 4];
 #pragma unroll
       for (int q = 0; q < KQ; ++q) {
@@ -276,7 +294,7 @@ __device__ __forceinline__ void b2_ang_force_pairs(
           Wp[4 * q + r] = fmaf(gp, wq[r], Wp[4 * q + r]);
         }
       }
-    }
+    });
     const float xh = x12 * dinv, yh = y12 * dinv, zh = z12 * dinv;
     float B[B2_NABC];
     b2_harmonics(xh, yh, zh, B);
@@ -378,7 +396,7 @@ __global__ void __launch_bounds__(128, 3) k_force_angular2(
     }
   }
   // ---- pairs ----
-  b2_ang_force_pairs<NT, K1, ORTHO>(P, p0, pz, box, i, b2_rec_load(p0, p1, i), w, ctab_s, arev);
+  b2_ang_force_pairs<NT, K1, ORTHO, B2AngShapeRT>(P, p0, pz, box, i, b2_rec_load(p0, p1, i), w, ctab_s, arev);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -386,21 +404,40 @@ __global__ void __launch_bounds__(128, 3) k_force_angular2(
 // one thread, for models that fit its budget (b2_fused_smem_bytes, DIMP = 32; nep_setup).  Nothing in
 // the chain depends on another atom's result, so s[n][abc], dU/dq and dU/ds stay on the SM:
 //   1. descriptor (b2_ang_desc_atom): s goes to the thread's shared-memory row, the angular components
-//      of q to the SoA columns P.q (they stay observable, b200md_nep_export_descriptors; the thread
-//      reads them back at once, from L2);
+//      of q to the SoA columns P.q (they stay observable, b200md_nep_export_descriptors);
 //   2. hidden layer (b2_mlp_core) from the radial part of q that k_desc_radial2 wrote and the angular
 //      part, weights from a shared-memory copy; site energy to acc[i];
 //   3. U table rows (b2_utable_compact) from the radial part of dU/dq;
 //   4. weights dU/ds (b2_ang_weights) in place over s;
 //   5. pair loop (b2_ang_force_pairs): f12 and arev.
 // Every step calls the body the five-kernel path calls, so the results are bit-identical to it with the
-// SIMT hidden layer.  dU/dq is copied to a thread-local array because steps 3 and 4 index it at run time
-// (nr1, na1 are model values); that array lives in local memory, which L1 / L2 cache.
+// SIMT hidden layer.  SH (B2AngShape) is the model's angular shape: with a fixed one the channel loops
+// unroll, dU/dq and q are indexed with constants, and the angular components of q reach the hidden layer
+// from registers instead of being read back from P.q.  B2AngShapeRT takes the shape from the model at run
+// time (every other model within the budget).
 // Dynamic shared memory: 128 rows of b2_ang_ws4(na1) float4s, the coefficient table, then w0 of each
 // type at a stride of b2_fused_w0_stride4 float4s (odd: a warp holding both types reads the two rows
 // on distinct banks), b0 and w1.
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ constexpr int b2_fused_w0_stride4(int nneu, int dimp) { return (nneu * dimp / 4) | 1; }
+
+#ifdef B2_FUSED_STOP
+// Diagnostic builds only (build_lib(variant=..., defs=["B2_FUSED_STOP=k"])): k_angular_fused returns after
+// step k (1 descriptor, 2 hidden layer, 3 U table, 4 weights) so that the stage profiler times the steps
+// before it.  f12 and arev of the atom's pairs are zeroed, so k_force_final2 reads valid slots; the forces
+// are then wrong, which is why no default build contains this.
+#define B2_FUSED_MAYBE_STOP(k, ...)                                           \
+  if (B2_FUSED_STOP == (k)) {                                                 \
+    __VA_ARGS__;                                                              \
+    for (int m = 0; m < P.nn_a[i]; ++m) {                                     \
+      reinterpret_cast<float4*>(P.f12)[(unsigned)m * N + i] = make_float4(0.f, 0.f, 0.f, 0.f); \
+      arev[(unsigned)m * N + i] = 0;                                          \
+    }                                                                         \
+    return;                                                                   \
+  }
+#else
+#define B2_FUSED_MAYBE_STOP(k, ...)
+#endif
 
 __host__ __device__ constexpr size_t b2_fused_smem_bytes(int nt, int na1, int k1a, int nneu, int dimp)
 {
@@ -408,7 +445,7 @@ __host__ __device__ constexpr size_t b2_fused_smem_bytes(int nt, int na1, int k1
          (size_t)nt * b2_fused_w0_stride4(nneu, dimp) * 16 + (size_t)2 * nt * nneu * 4;
 }
 
-template <int NT, int K1, int DIMP, bool ORTHO>
+template <int NT, int K1, int DIMP, bool ORTHO, class SH>
 __global__ void __launch_bounds__(128, 3) k_angular_fused(
   const B2NepView P, const int4* __restrict__ p0, const int4* __restrict__ p1,
   const double* __restrict__ pz, const B2Box box, int* __restrict__ arev)
@@ -416,7 +453,7 @@ __global__ void __launch_bounds__(128, 3) k_angular_fused(
   static_assert(NT == 1 || NT == 2, "few-type path");
   constexpr int KQ = (K1 + 3) / 4;
   extern __shared__ float4 af_smem[];
-  const int na1 = P.na1, nneu = P.nneu;
+  const int na1 = SH::na1(P), nr1 = SH::nr1(P), nneu = P.nneu;
   const int WS4 = b2_ang_ws4(na1);
   float4* const ctab_s = af_smem + blockDim.x * WS4;
   float4* const w0_s = ctab_s + P.nt * P.nt * na1 * KQ;
@@ -443,35 +480,51 @@ __global__ void __launch_bounds__(128, 3) k_angular_fused(
   const unsigned N = (unsigned)P.n;
   float4* const row = af_smem + threadIdx.x * WS4;
   const B2Rec a1 = b2_rec_load(p0, p1, i);
-  // 1. descriptor
-  b2_ang_desc_atom<NT, K1, 3, ORTHO>(
-    P, p0, pz, box, i, a1, ctab_s, [&](int k, float v) { P.q[(size_t)k * N + i] = v; },
+  // 1. descriptor; with a fixed shape the angular components of q also stay in q[] for step 2
+  float q[DIMP];
+  b2_ang_desc_atom<NT, K1, 3, ORTHO, SH>(
+    P, p0, pz, box, i, a1, ctab_s,
+    [&](int k, float v) {
+      P.q[(size_t)k * N + i] = v;
+      if constexpr (SH::fixed)
+        q[k] = v;
+    },
     [&](int g, float4 v) { row[g] = v; });
+  B2_FUSED_MAYBE_STOP(1, );
   // 2. hidden layer
   const int t = a1.t;
-  float fl[DIMP]; // dU/dq, indexed at run time below
+  float fl[DIMP]; // dU/dq
   {
-    float q[DIMP], Fp[DIMP];
+    float Fp[DIMP];
 #pragma unroll
-    for (int d = 0; d < DIMP; ++d)
-      q[d] = (d < P.dim) ? P.q[(size_t)d * N + i] * __ldg(&P.q_scaler[d]) : 0.0f;
-    const float F = b2_mlp_core<DIMP, false>(q, w0_s + t * wst4, b0_s + t * nneu, w1_s + t * nneu, nneu,
-                                             __ldg(&P.bias[t]), P.q_scaler, Fp);
+    for (int d = 0; d < DIMP; ++d) {
+      if (d < SH::dim(P))
+        q[d] = (SH::fixed && d >= nr1 ? q[d] : P.q[(size_t)d * N + i]) * __ldg(&P.q_scaler[d]);
+      else
+        q[d] = 0.0f;
+    }
+    // paired neurons only on a fixed shape: the run-time-shape instance measured slower with them
+    const float F = b2_mlp_core<DIMP, false, SH::fixed>(q, w0_s + t * wst4, b0_s + t * nneu,
+                                                        w1_s + t * nneu, nneu, __ldg(&P.bias[t]),
+                                                        P.q_scaler, Fp);
     P.acc[i] = (double)F;
 #pragma unroll
     for (int d = 0; d < DIMP; ++d)
       fl[d] = Fp[d];
   }
+  B2_FUSED_MAYBE_STOP(2, for (int d = 0; d < DIMP; ++d) asm volatile("" ::"f"(fl[d])));
   // 3. U table
   auto fr = [&](int n) { return fl[n]; };
   switch (P.K1R) {
-    case 9: b2_utable_compact<9>(P, i, t, fr); break;
-    case 13: b2_utable_compact<13>(P, i, t, fr); break;
-    default: b2_utable_compact<17>(P, i, t, fr); break;
+    case 9: b2_utable_compact<9, SH::nr1_const>(P, i, t, fr); break;
+    case 13: b2_utable_compact<13, SH::nr1_const>(P, i, t, fr); break;
+    default: b2_utable_compact<17, SH::nr1_const>(P, i, t, fr); break;
   }
+  B2_FUSED_MAYBE_STOP(3, for (int d = 0; d < DIMP; ++d) asm volatile("" ::"f"(fl[d])));
   // 4. weights over s
-  const float* fa = fl + P.nr1;
-  for (int n = 0; n < na1; ++n) {
+  const float* fa = fl + nr1;
+  const int h222 = SH::has222(P), h1111 = SH::has1111(P);
+  b2_channel_loop<SH::fixed>(na1, 1, [&](int n) {
     float s[B2_NABC];
 #pragma unroll
     for (int g = 0; g < B2_ABC4; ++g) {
@@ -485,16 +538,17 @@ __global__ void __launch_bounds__(128, 3) k_angular_fused(
 #pragma unroll
     for (int L = 0; L < 4; ++L)
       F6[L] = fa[L * na1 + n];
-    F6[4] = P.has222 ? fa[4 * na1 + n] : 0.0f;
-    F6[5] = P.has1111 ? fa[(4 + (P.has222 ? 1 : 0)) * na1 + n] : 0.0f;
+    F6[4] = h222 ? fa[4 * na1 + n] : 0.0f;
+    F6[5] = h1111 ? fa[(4 + (h222 ? 1 : 0)) * na1 + n] : 0.0f;
     float wv[B2_NABC];
-    b2_ang_weights(s, F6, P.has222, P.has1111, wv);
+    b2_ang_weights(s, F6, h222, h1111, wv);
 #pragma unroll
     for (int g = 0; g < B2_ABC4; ++g)
       row[n * B2_ABC4 + g] = make_float4(wv[4 * g], wv[4 * g + 1], wv[4 * g + 2], wv[4 * g + 3]);
-  }
+  });
+  B2_FUSED_MAYBE_STOP(4, );
   // 5. pairs
-  b2_ang_force_pairs<NT, K1, ORTHO>(P, p0, pz, box, i, a1, row, ctab_s, arev);
+  b2_ang_force_pairs<NT, K1, ORTHO, SH>(P, p0, pz, box, i, a1, row, ctab_s, arev);
 }
 
 } // namespace b2

@@ -205,6 +205,12 @@ class NEP(Potential):
         return q.cpu().numpy()
 
     @property
+    def fused_shape(self):
+        """Instance of k_angular_fused the potential runs: 0 none (separate angular kernels), 1 the run-time
+        shape, 2 / 3 n_max 4 4 with l_max 4 2 0 / 4 0 0 compiled in."""
+        return self._L.b200md_nep_info(self._h, 10)
+
+    @property
     def num_tiles(self):
         """Type tiles of the last list rebuild (0: the SIMT hidden layer has none)."""
         return self._L.b200md_nep_info(self._h, 8)

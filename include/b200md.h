@@ -53,7 +53,9 @@ void b200md_nep_destroy(b200md_nep* p);
  * (enlarged), 5 zbl enabled, 6 number of neighbour-list rebuilds so far, 7 segments of the warp
  * schedule (0: identity schedule, see b200md_nep_export_schedule), 8 type tiles of the last list rebuild
  * (0: no tiles, the SIMT hidden layer), 9 CTAs of the last launch of the tensor-core hidden layer (0: the
- * last compute did not run it).  6 and 8 synchronise the device. */
+ * last compute did not run it), 10 angular shape of k_angular_fused (0: the separate angular kernels run,
+ * 1: the run-time-shape instance, 2: n_max 4 4 with l_max 4 2 0 compiled in, 3: the same with l_max 4 0 0).
+ * 6 and 8 synchronise the device. */
 int b200md_nep_info(const b200md_nep* p, int what);
 double b200md_nep_rc(const b200md_nep* p); /* Potential::rc, src/force/potential.cuh:32 */
 /* atomic symbol of type t (species -> type index mapping, src/model/read_xyz.cu:349-361) */
