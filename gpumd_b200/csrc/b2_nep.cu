@@ -406,6 +406,7 @@ struct b200md_nep {
   bool rad_direct = false; // many types: contract every pair on the spot (k_desc_radial<-1,...>), see nep_setup
   bool rad_reg = false;   // 3..16 types: radial accumulators in registers (k_desc_radial<4|8|16,...>); slower
                           // than the shared-memory accumulators on UNEP-v1, B200MD_NEP_RADREG=1
+  int rad_nt = 0;         // 3+ types: NT of the k_desc_radial instance (-1, 0, 4, 8, 16), see nep_setup
   bool ang_cstage = true; // k_desc_angular: coefficient table staged in shared memory
   bool radial_v2 = false; // few-type radial passes of b2_nep_radial.cuh (planes, branch-free loop)
   bool sched = false;     // their warps follow Neighbor::seg_order (B200MD_NEP_SCHED=0: identity, A/B runs)
@@ -478,10 +479,7 @@ int dispatch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
   } else if (p->model.nt == 2) {
     return launch_desc_radial<2, K1, true>(p, box, st);
   } else {
-    // 3..16 types: register accumulators when NT*K1 fits the register file are an opt-in
-    // (B200MD_NEP_RADREG=1); the default keeps the accumulators in shared memory
-    const int nt = p->model.nt;
-    const int ntb = !p->rad_reg ? 0 : nt <= 4 ? 4 : nt <= 8 ? 8 : nt <= 16 ? 16 : 0;
+    // 3+ types: the instance nep_setup chose (p->rad_nt)
     if (!p->fuse_split) {
       k_split<<<grid_for(p->n, BLK), BLK, 0, st>>>(p->view, box);
       B2_LAUNCHED();
@@ -489,16 +487,16 @@ int dispatch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 #define B2_DR(NT_)                                                 \
   return p->fuse_split ? launch_desc_radial<NT_, K1, true>(p, box, st) \
                        : launch_desc_radial<NT_, K1, false>(p, box, st)
-    if (p->rad_direct)
+    if (p->rad_nt == -1)
       B2_DR(-1);
-    if (ntb == 4)
+    if (p->rad_nt == 4)
       B2_DR(4);
     if constexpr (8 * K1 <= 160) {
-      if (ntb == 8)
+      if (p->rad_nt == 8)
         B2_DR(8);
     }
     if constexpr (16 * K1 <= 160) {
-      if (ntb == 16)
+      if (p->rad_nt == 16)
         B2_DR(16);
     }
     B2_DR(0);
@@ -608,6 +606,18 @@ int launch_angular2(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool
   return B200MD_OK;
 }
 
+// k_desc_angular's coefficient table: float4 rows of (na1 * KQ) | 1, one per type pair
+int ang_coeff_row(const b200md_nep* p) { return (p->model.na1 * ((p->model.K1A + 3) / 4)) | 1; }
+
+size_t ang_coeff_bytes(const b200md_nep* p)
+{
+  return (size_t)p->model.nt * p->model.nt * ang_coeff_row(p) * sizeof(float4);
+}
+
+// shared-memory copy of the angular coefficients when three blocks of it fit an SM
+// (B200MD_NEP_CSTAGE=0: read them from global memory)
+bool ang_coeff_staged(const b200md_nep* p) { return p->ang_cstage && ang_coeff_bytes(p) <= 72 * 1024; }
+
 template <int K1>
 int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool force)
 {
@@ -622,12 +632,9 @@ int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool 
   }
   if (!force) {
     {
-      // shared-memory copy of the angular coefficients when three blocks of it fit an SM
-      // (B200MD_NEP_CSTAGE=0: read them from global memory)
-      constexpr int KQ = (K1 + 3) / 4;
-      const int rs4 = (p->model.na1 * KQ) | 1;
-      const size_t bytes = (size_t)p->model.nt * p->model.nt * rs4 * sizeof(float4);
-      const bool stage = p->ang_cstage && bytes <= 72 * 1024;
+      const int rs4 = ang_coeff_row(p);
+      const size_t bytes = ang_coeff_bytes(p);
+      const bool stage = ang_coeff_staged(p);
       auto kern = k_desc_angular<K1, 5>;
       if (stage && bytes > 48 * 1024)
         B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
@@ -683,11 +690,19 @@ int launch_angular_fused(const b200md_nep* p, const B2Box& box, cudaStream_t st)
   }
 }
 
+// k_mlp's weights of every type in shared memory (STAGE = true) while they fit 96 KB
+size_t mlp_weight_bytes(const b200md_nep* p)
+{
+  return (size_t)p->model.nt * p->model.nneu * (p->model.DIMP + 2) * sizeof(float);
+}
+
+bool mlp_weights_staged(const b200md_nep* p) { return mlp_weight_bytes(p) <= 96 * 1024; }
+
 template <int DIMP>
 int launch_mlp(const b200md_nep* p, cudaStream_t st)
 {
-  const size_t bytes = (size_t)p->model.nt * p->model.nneu * (DIMP + 2) * sizeof(float);
-  if (bytes <= 96 * 1024) {
+  const size_t bytes = mlp_weight_bytes(p);
+  if (mlp_weights_staged(p)) {
     auto kern = k_mlp<DIMP, true>;
     if (bytes > 48 * 1024)
       B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
@@ -1058,6 +1073,13 @@ int nep_setup(b200md_nep* p, int num_atoms)
       P.c_r4 = reinterpret_cast<const float4*>(p->c_r4.p); // regardless of B200MD_NEP_CVEC
     }
   }
+  // 3..16 types: register accumulators (B200MD_NEP_RADREG=1) when NT*K1 fits the register file; the
+  // default keeps the accumulators in shared memory
+  {
+    const int nt = m.nt;
+    const int ntb = !p->rad_reg ? 0 : nt <= 4 ? 4 : nt <= 8 ? 8 : nt <= 16 ? 16 : 0;
+    p->rad_nt = p->rad_direct ? -1 : ntb * m.K1R <= 160 ? ntb : 0;
+  }
   B2_CUDA(cudaDeviceSynchronize());
   return B200MD_OK;
 }
@@ -1130,6 +1152,33 @@ int b200md_nep_info(const b200md_nep* p, int what)
     case 8: return nep_tile_count(p);
     case 9: return p->tc_ctas_last;
     case 10: return p->fused_shape;
+    case 11: return p->ang_fused ? 0 : p->ang_block;
+    case 12: { // mirrors dispatch_desc_radial
+      const int nt = p->model.nt;
+      if (p->view.team)
+        return 200 + nt;
+      if (p->radial_v2)
+        return 100 + nt;
+      return nt <= 2 ? nt : p->rad_nt;
+    }
+    case 13:
+      if (p->view.team || p->radial_v2)
+        return -1;
+      return (p->model.nt <= 2 || p->fuse_split) ? 1 : 0;
+    case 14:
+      if (p->ang_fused)
+        return 0;
+      return (p->use_tc && p->view.N3) ? 1 : 2;
+    case 15:
+      if (p->radial_v2)
+        return -1;
+      return ang_coeff_staged(p) ? 1 : 0;
+    case 16: return p->rev_slot ? 1 : 0;
+    case 17: return (p->ang_fused || p->use_tc) ? 0 : p->model.DIMP;
+    case 18:
+      if (p->ang_fused || p->use_tc)
+        return -1;
+      return mlp_weights_staged(p) ? 1 : 0;
     default: return -1;
   }
 }

@@ -220,6 +220,16 @@ class NEP(Potential):
         """CTAs of the last tensor-core hidden-layer launch (0: the last compute did not run it)."""
         return self._L.b200md_nep_info(self._h, 9)
 
+    @property
+    def instances(self):
+        """The kernel instances the potential runs (b200md_nep_info 11-18, include/b200md.h): ang_block (threads
+        per block of the angular force kernel), radial_nt (NT of k_desc_radial; 100 / 200 + types for the
+        plane-based / lane-team kernels of one and two types), split (1 fused, 0 k_split, -1 none), utable
+        (1 tensor-core GEMM, 2 k_utable, 0 none), cstage (k_desc_angular's coefficients in shared memory 1,
+        global 0, -1 not run), revslot, mlp_dimp and mlp_stage (k_mlp<DIMP, STAGE>; 0 / -1: not run)."""
+        keys = ("ang_block", "radial_nt", "split", "utable", "cstage", "revslot", "mlp_dimp", "mlp_stage")
+        return {k: self._L.b200md_nep_info(self._h, 11 + i) for i, k in enumerate(keys)}
+
     def export_tiles(self, n=None):
         """(slot[n] of every caller-order atom, tile_type[num_tiles]) of the last list rebuild."""
         n = n or self.N2

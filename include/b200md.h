@@ -55,6 +55,21 @@ void b200md_nep_destroy(b200md_nep* p);
  * (0: no tiles, the SIMT hidden layer), 9 CTAs of the last launch of the tensor-core hidden layer (0: the
  * last compute did not run it), 10 angular shape of k_angular_fused (0: the separate angular kernels run,
  * 1: the run-time-shape instance, 2: n_max 4 4 with l_max 4 2 0 compiled in, 3: the same with l_max 4 0 0).
+ * The kernel instances the handle runs:
+ *   11 threads per block of the angular force kernel (128, 64 or 32; 0: k_angular_fused runs instead)
+ *   12 radial descriptor kernel: for three or more types NT of k_desc_radial<NT, K1, SPLIT> (-1 per-pair
+ *      contraction, 0 accumulators in shared memory, 4 / 8 / 16 accumulators in registers); for one or two
+ *      types 100 + types (the plane-based kernels), 200 + types (the lane-team kernels) or the number of
+ *      types (the generic thread-per-atom instance)
+ *   13 SPLIT of that k_desc_radial instance (1: the neighbour split is fused into it, 0: k_split runs
+ *      before it; -1: the one- and two-type kernels, which have no split)
+ *   14 the U table comes from the tensor-core hidden layer's third GEMM (1), from k_utable (2), or is not
+ *      stored (0: k_angular_fused)
+ *   15 k_desc_angular reads its coefficient table from shared memory (1) or global memory (0); -1: the
+ *      one- and two-type angular kernels run instead
+ *   16 direct reverse slots in the angular pair reduction (1: B200MD_NEP_REVSLOT=1 is in effect)
+ *   17 DIMP of the SIMT hidden layer k_mlp<DIMP, STAGE> (0: the tensor-core layer or k_angular_fused)
+ *   18 STAGE of that k_mlp instance (1: weights in shared memory, 0: in global memory; -1: it does not run)
  * 6 and 8 synchronise the device. */
 int b200md_nep_info(const b200md_nep* p, int what);
 double b200md_nep_rc(const b200md_nep* p); /* Potential::rc, src/force/potential.cuh:32 */

@@ -304,6 +304,14 @@ def main():
         s = fcc(8, 3.1, rattle=0.15, seed=61, num_types=2, symbols=("Ar", "Ar"))
         d, i = run_case(name, s, sym, GOLDEN / model, sp)
         collect_single_point(d, s, sym); infos.append(i)
+    # the same for three and four species: typewise ZBL over Li / Mg / Al / Si, and NEP5 with the six rows of a
+    # flexible ZBL table (tests/test_many_species_cpu.py)
+    for name, model in (("sp_4sp_typewise_zbl", "nep_synth_4sp_typewise_zbl.txt"),
+                        ("sp_3sp_nep5_flexzbl", "nep_synth_3sp_nep5_flexzbl.txt")):
+        sym = nep_type_order(GOLDEN / model)
+        s = fcc(8, 3.1, rattle=0.15, seed=62, num_types=len(sym), symbols=("Ar",) * len(sym))
+        d, i = run_case(name, s, sym, GOLDEN / model, sp)
+        collect_single_point(d, s, sym); infos.append(i)
 
     # LJ / Tersoff / EAM beyond one orthogonal, periodic, few-species crystal (tests/cases_classical.py):
     # per-pair LJ tables in a triclinic box, the Tersoff SiC mixing rules (also with an open direction),

@@ -5,7 +5,7 @@ Everything copied here is DATA the reference's own tests/examples pin this path 
 No reference source code is copied.  /root/reference does not exist on the GPU box, so the
 tests only ever read the committed copies.
 
-    python tests/golden/make_fixtures.py [few_species]
+    python tests/golden/make_fixtures.py [few_species | many_species]
 """
 import gzip
 import shutil
@@ -80,6 +80,7 @@ def main():
     print("wrote carbon_model.npz", pos.shape)
     nep_cpu_goldens()
     nep_cpu_goldens_few_species()
+    nep_cpu_goldens_many_species()
 
 
 def nep_cpu_goldens():
@@ -119,8 +120,28 @@ def nep_cpu_goldens_few_species():
     print("wrote ref_nep_cpu_few_species.npz", sorted(out))
 
 
+def nep_cpu_goldens_many_species():
+    """The same for the synthetic models of three to sixteen species NEP_CPU reads: inputs of
+    tests/test_many_species_cpu.py::test_oracle_matches_reference_nep_cpu_many_species."""
+    root = OUT.parents[1]
+    sys.path[:0] = [str(root), str(root / "tests")]
+    from oracle import oracle_py
+    from test_many_species_cpu import MANY_SPECIES_CASES, NEP_CPU_MANY_SPECIES, nep_cpu_many_species_structure
+    assert oracle_py.ref_available(), "oracle/_ref/libnep_cpu_ref.so not built"
+    out = {}
+    for case in NEP_CPU_MANY_SPECIES:
+        s = nep_cpu_many_species_structure(case)
+        r = oracle_py.RefNepCpu(OUT / MANY_SPECIES_CASES[case][0]).compute(s["type"], s["h"], s["pos"])
+        for k in ("pe", "force", "virial"):
+            out[f"{case}_{k}"] = np.asarray(r[k], dtype=np.float64)
+    np.savez_compressed(OUT / "ref_nep_cpu_many_species.npz", **out)
+    print("wrote ref_nep_cpu_many_species.npz", sorted(out))
+
+
 if __name__ == "__main__":
     if sys.argv[1:] == ["few_species"]:  # only the NEP_CPU results of the synthetic few-species models
         nep_cpu_goldens_few_species()
+    elif sys.argv[1:] == ["many_species"]:  # ... of the synthetic models of three or more species
+        nep_cpu_goldens_many_species()
     else:
         main()

@@ -27,20 +27,29 @@ def check_fv(out, ref, noise=1.0, gap_f=0.0, gap_v=0.0):
                  atol=TOL["virial"]["atol"] * vs + gap_v, what="virial")
 
 
-def check_nep(oracle, dev, model, s, n, energy_tol=None):
+def check_nep(oracle, dev, model, s, n, energy_tol=None, q_gap=False):
     """energy_tol: eV/atom bound against the FP32 restatement (default 1e-6, SURVEY 8d).  Callers with
-    deep-well models (|E|/N of several eV) pass 1e-6 * |E|/N: FP32 rounding is relative."""
+    deep-well models (|E|/N of several eV) pass 1e-6 * |E|/N: FP32 rounding is relative.
+    q_gap: for models with ~300 radial neighbours (rc = 8 A), whose FP32 radial sums cancel to 1e-5 of their
+    terms: each descriptor component's atol gets twice the FP32 restatement's own largest distance from the
+    FP64 descriptors (another FP32 summation order may sit on the other side of the FP64 value), and the
+    descriptors are also checked against FP64."""
     energy_tol = TOL["energy_per_atom"] if energy_tol is None else energy_tol
     orc = oracle.NepOracle(GOLDEN / model)
     r32 = orc.compute(s["type"], s["h"], s["pbc"], s["pos"], precision=32, lists=True, descriptors=True)
-    r64 = orc.compute(s["type"], s["h"], s["pbc"], s["pos"], precision=64)
+    r64 = orc.compute(s["type"], s["h"], s["pbc"], s["pos"], precision=64, descriptors=q_gap)
     rc, out = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc == 0
     NNr, NLr, NNa, NLa = dev.neighbors(r32["NL_radial"].shape[1], r32["NL_angular"].shape[1])
     assert np.array_equal(NNr, r32["NN_radial"]) and np.array_equal(NLr, r32["NL_radial"])
     assert np.array_equal(NNa, r32["NN_angular"]) and np.array_equal(NLa, r32["NL_angular"])
     q = dev.descriptors(orc.info["dim"])
-    assert_close(q, r32["q"], rtol=2e-5, atol=2e-6, what="descriptor")
+    if q_gap:
+        q_atol = 2e-6 + 2 * np.abs(r32["q"] - r64["q"]).max(axis=1, keepdims=True)
+        assert_close(q, r64["q"], rtol=2e-5, atol=q_atol, what="descriptor vs FP64")
+    else:
+        q_atol = 2e-6
+    assert_close(q, r32["q"], rtol=2e-5, atol=q_atol, what="descriptor")
     # |dE|/N <= 1e-6 eV against the FP32 restatement (the reference GPU's arithmetic); against the
     # FP64 truth allow the FP32 pair-math noise itself (the restatement's own f32-f64 gap) on top
     gap = abs(r32["pe"].sum() - r64["pe"].sum()) / n
