@@ -821,14 +821,14 @@ class Ensemble_BAO(Ensemble_LAN):
 class Ensemble_BDP(Ensemble_NVE):
     """nvt_bdp, src/integrate/ensemble_bdp.cu:69-101: velocity-Verlet, thermo, then the stochastic
     rescaling of Bussi et al.; generator and factor live on the device (seed 12345678 = the
-    reference's -DDEBUG stream)."""
+    reference's -DDEBUG stream).  The generator is created at the first compute2, after set_groups:
+    its degrees of freedom are ndeg = 3 (N - N_fixed - N_move) (ensemble_bdp.cu:87-95)."""
+
+    _bdp = None
 
     def __init__(self, num_atoms, temperature, temperature_coupling, seed=12345678):
         super().__init__(num_atoms)
-        h = C.c_void_p()
-        _lib.check(self._L.b200md_bdp_create(int(num_atoms), float(temperature),
-                                             float(temperature_coupling), int(seed), C.byref(h)))
-        self._bdp = h
+        self._args = (float(temperature), float(temperature_coupling), int(seed))
 
     def __del__(self):
         if getattr(self, "_bdp", None):
@@ -838,6 +838,11 @@ class Ensemble_BDP(Ensemble_NVE):
     def compute2(self, time_step, box, atom, thermo):
         super().compute2(time_step, box, atom, thermo)
         n = atom.number_of_atoms
+        if self._bdp is None:
+            h = C.c_void_p()
+            _lib.check(self._L.b200md_bdp_create(n - getattr(self, "_n_excluded", 0), *self._args,
+                                                 C.byref(h)))
+            self._bdp = h
         _lib.check(self._L.b200md_bdp_step(
             self._bdp, n, n, _ptr(thermo), _ptr(atom.velocity_per_atom), _stream()))
 

@@ -33,16 +33,21 @@ void B200_Integrator::b2_velocity_verlet(
     b2h_fail("Ensemble::velocity_verlet");
 }
 
+int B200_Integrator::b2_num_integrated(const Ensemble& e, const std::vector<Group>& group, int n)
+{
+  if (e.fixed_group >= 0)
+    n -= group[e.fixed_grouping_method].cpu_size[e.fixed_group];
+  if (e.move_group >= 0)
+    n -= group[e.move_grouping_method].cpu_size[e.move_group];
+  return n;
+}
+
 void B200_Integrator::b2_find_thermo(
   const Ensemble& e, const double volume, const std::vector<Group>& group, Atom& atom,
   GPU_Vector<double>& thermo)
 {
   const int n = atom.number_of_atoms;
-  int n_temperature = n; // ensemble.cu:645-651
-  if (e.fixed_group >= 0)
-    n_temperature -= group[e.fixed_grouping_method].cpu_size[e.fixed_group];
-  if (e.move_group >= 0)
-    n_temperature -= group[e.move_grouping_method].cpu_size[e.move_group];
+  const int n_temperature = b2_num_integrated(e, group, n); // ensemble.cu:645-651
   const size_t need = (size_t)b200md_thermo_scratch_bytes(n);
   if (scratch_.size() != need)
     scratch_.resize(need, 0);
@@ -123,15 +128,13 @@ void Ensemble_BER_B200::compute2(
   }
 }
 
-Ensemble_BDP_B200::Ensemble_BDP_B200(
-  int t, int mg, const double mv[3], int N, double T, double Tc, unsigned seed)
+Ensemble_BDP_B200::Ensemble_BDP_B200(int t, int mg, const double mv[3], double T, double Tc, unsigned seed)
 {
   type = t;
   temperature = T;
   temperature_coupling = Tc;
   set_move(*this, mg, mv);
-  if (b200md_bdp_create(N, T, Tc, seed, &bdp_) != B200MD_OK)
-    b2h_fail("Ensemble_BDP_B200");
+  seed_ = seed;
 }
 
 Ensemble_BDP_B200::~Ensemble_BDP_B200() { b200md_bdp_destroy(bdp_); }
@@ -149,6 +152,12 @@ void Ensemble_BDP_B200::compute2(
   b2_velocity_verlet(*this, false, time_step, group, atom);
   b2_find_thermo(*this, box.get_volume(), group, atom, thermo);
   const int n = atom.number_of_atoms;
+  // the first step: `fix` / `move` are set by now (integrate.cu:279-281), so the generator gets
+  // ndeg = 3 (N - N_fixed - N_move) (ensemble_bdp.cu:87-95); the seed is fixed, so creating it
+  // here rather than in the constructor leaves the stream unchanged
+  if (!bdp_ && b200md_bdp_create(b2_num_integrated(*this, group, n), temperature, temperature_coupling,
+                                 seed_, &bdp_) != B200MD_OK)
+    b2h_fail("Ensemble_BDP_B200");
   if (b200md_bdp_step(bdp_, n, n, thermo.data(), atom.velocity_per_atom.data(), nullptr) != B200MD_OK)
     b2h_fail("Ensemble_BDP_B200::compute2");
 }

@@ -51,6 +51,8 @@ protected:
   void b2_velocity_verlet(
     const Ensemble& e, const bool is_step1, const double time_step, const std::vector<Group>& group,
     Atom& atom);
+  // the atoms outside the fixed and moving groups, ensemble.cu:645-651 and ensemble_bdp.cu:87-88
+  static int b2_num_integrated(const Ensemble& e, const std::vector<Group>& group, int n);
   // Ensemble::find_thermo (ensemble.cu:636-673): fixed / moving atoms do not count for T
   void b2_find_thermo(
     const Ensemble& e, const double volume, const std::vector<Group>& group, Atom& atom,
@@ -127,11 +129,13 @@ private:
   double c1_ = 0.0;
 };
 
-// the generator lives on the device; seed 12345678 follows the reference's -DDEBUG stream
+// the generator lives on the device; seed 12345678 follows the reference's -DDEBUG stream.  It is
+// created at the first compute2, when `fix` / `move` are known: its degrees of freedom are
+// ndeg = 3 (N - N_fixed - N_move) (ensemble_bdp.cu:87-95)
 class Ensemble_BDP_B200 : public Ensemble, protected B200_Integrator
 {
 public:
-  Ensemble_BDP_B200(int t, int mg, const double mv[3], int N, double T, double Tc, unsigned seed = 12345678u);
+  Ensemble_BDP_B200(int t, int mg, const double mv[3], double T, double Tc, unsigned seed = 12345678u);
   ~Ensemble_BDP_B200() override;
   void compute1(
     const double time_step, const std::vector<Group>& group, Box& box, Atom& atom,
@@ -142,6 +146,7 @@ public:
 
 private:
   b200md_bdp* bdp_ = nullptr;
+  unsigned seed_ = 0;
 };
 
 class Ensemble_NHC_B200 : public Ensemble, protected B200_Integrator

@@ -693,7 +693,16 @@ private:
     } else if (e.type == 1) {
       ensemble_.reset(new Ensemble_BER_B200(1, move_group_, move_velocity_, e.T, e.Tc));
     } else if (e.type == 4) {
-      ensemble_.reset(new Ensemble_BDP_B200(4, move_group_, move_velocity_, N, e.T, e.Tc,
+      // the thermostat's degrees of freedom are ndeg = 3 (N - N_fixed - N_move) (ensemble_bdp.cu:87-95,
+      // counted by Ensemble_BDP_B200 at its first step): at least one atom must be integrated
+      int n_integrated = N;
+      if (fixed_group_ >= 0)
+        n_integrated -= model_.group[fixed_method_].cpu_size[fixed_group_];
+      if (move_group_ >= 0)
+        n_integrated -= model_.group[move_method_].cpu_size[move_group_];
+      if (n_integrated < 1)
+        input_error("nvt_bdp needs at least one atom outside the fixed and moving groups.");
+      ensemble_.reset(new Ensemble_BDP_B200(4, move_group_, move_velocity_, e.T, e.Tc,
                                             e.has_seed ? e.seed : bdp_seed()));
     } else if (e.type == 3) {
       ensemble_.reset(new Ensemble_LAN_B200(3, N, e.T, e.Tc, (unsigned long long)rand())); // ensemble_lan.cu:39

@@ -64,7 +64,7 @@ bool b200md_make_ensemble(
       const unsigned seed = (unsigned)std::chrono::system_clock::now().time_since_epoch().count();
 #endif
       ensemble.reset(new Ensemble_BDP_B200(
-        type, move_group, move_velocity, number_of_atoms, temperature, temperature_coupling, seed));
+        type, move_group, move_velocity, temperature, temperature_coupling, seed));
       break;
     }
     case 3: // the reference seeds cuRAND with rand() (ensemble_lan.cu:39): same call, same stream

@@ -246,8 +246,9 @@ int b200md_scale_velocity(int n, double factor, double* d_velocity, void* stream
  *                                   svr_utilities.cuh:27-135): stochastic velocity rescaling after
  *                                   the second half step.  The generator (std::mt19937 semantics)
  *                                   lives on the device; seed 12345678 reproduces the reference's
- *                                   -DDEBUG stream (ensemble_bdp.cu:31-32).  3*n_global must fit an
- *                                   int, as in the reference. */
+ *                                   -DDEBUG stream (ensemble_bdp.cu:31-32).  n_global counts the atoms
+ *                                   that are integrated, N - N_fixed - N_move: ndeg = 3*n_global
+ *                                   (ensemble_bdp.cu:87-95) must fit an int, as in the reference. */
 int b200md_berendsen_temperature(
   int n, int stride, double temperature, double temperature_coupling, const double* d_thermo,
   double* d_velocity, void* stream);

@@ -395,6 +395,8 @@ class BdpOracle:
                 + 2.0 * rr * math.sqrt(kk * sigma / ndeg * (1.0 - factor) * factor))
 
     def factor(self, t_instant, n_atoms, temperature, temperature_coupling):
+        """n_atoms counts the atoms that are integrated, N - N_fixed - N_move: ndeg = 3 n_atoms
+        (ensemble_bdp.cu:87-95)."""
         ndeg = 3 * n_atoms
         ek = t_instant * ndeg * 8.617343e-5 * 0.5
         sigma = ndeg * 8.617343e-5 * temperature * 0.5
