@@ -1,14 +1,13 @@
 """LJ, Tersoff-1989 and EAM kernels on the device: triclinic, open and multi-species boxes against the FP32
 oracle and the FP64 references (tests/cases_classical.py), known-answer clusters, per-pair LJ cutoffs,
-skin-list reuse / rebuild / invalidation, NVE runs, block domains and the benchmark sizes."""
+skin-list reuse / rebuild / invalidation, NVE runs and block domains (the benchmark sizes: test_gpu_full_size.py)."""
 import numpy as np
 import pytest
 
 import cases_classical as cc
 from conftest import GOLDEN
-from gpumd_b200.structures import TIME_UNIT_CONVERSION, diamond, fcc, init_velocities
+from gpumd_b200.structures import TIME_UNIT_CONVERSION, fcc, init_velocities
 from test_classical_cpu import CLUSTERS, check_cluster, check_vs_fp64, check_vs_oracle, make_cluster
-from test_kernel_bodies_cpu import check_fv
 
 pytestmark = pytest.mark.gpu
 
@@ -288,41 +287,3 @@ def test_eam_blocks_follow_the_single_domain_trajectory(oracle, mg):
     assert pot.num_rebuilds >= 2  # the first build, then at least one triggered by the skin check
     assert abs(th[0] - rows[-1][0]) < 0.05 and abs(th[1] - rows[-1][1]) < 2e-6 * n
     check_vs_oracle(out, cc.oracle32("eam", CUFENI, dict(s, pos=out["pos"])), n, "eam", CUFENI)
-
-
-# ---------------------------------------------------------------- benchmark sizes
-
-@pytest.mark.parametrize("workload", ["lj", "si"])
-def test_full_size_properties(oracle, eng, workload):
-    """bench.py's --workload lj (1 000 188 Ar atoms) and si (2 000 376 Si atoms): finite outputs, sum of
-    forces ~ 0, a spatial sub-block against the oracle on that block's neighbourhood, bit-identical
-    repeat (test_gpu_md.test_full_size_properties_pbte_1m for LJ and Tersoff)."""
-    if workload == "lj":
-        kind, path, s = "lj", cc.LJ1, fcc(63, 5.30, rattle=0.05, seed=1)
-        halo, fsum = 10.0 + 1.0, 2e-3
-    else:
-        kind, path, s = "tersoff", cc.SI, diamond(63, a=5.431, rattle=0.05, seed=1)
-        halo, fsum = 2 * 3.0 + 1.0, 1e-8
-    n = s["type"].shape[0]
-    assert n == {"lj": 1_000_188, "si": 2_000_376}[workload]
-    out, pot = compute(eng, kind, path, s)
-    assert all(np.isfinite(out[k]).all() for k in ("pe", "force", "virial"))
-    assert np.abs(out["force"].sum(axis=1)).max() < fsum
-    pos = s["pos"]
-    d = pos - np.array([100.0, 120.0, 140.0])[:, None]
-    inner = np.nonzero((np.abs(d) < 6.0).all(axis=0))[0]
-    shell = np.nonzero((np.abs(d) < 6.0 + halo).all(axis=0))[0]
-    sub = dict(pos=np.ascontiguousarray(pos[:, shell]), type=s["type"][shell], h=s["h"], pbc=np.array([0, 0, 0], np.int32))
-    r = cc.oracle32(kind, path, sub)
-    w = np.searchsorted(shell, inner)
-    part = {k: out[k][..., inner] for k in ("pe", "force", "virial")}
-    ref = {k: r[k][..., w] for k in ("pe", "force", "virial")}
-    if kind == "tersoff":
-        np.testing.assert_allclose(part["force"], ref["force"], rtol=1e-9, atol=1e-10)
-        np.testing.assert_allclose(part["pe"], ref["pe"], rtol=1e-10, atol=1e-11)
-    else:
-        np.testing.assert_allclose(part["pe"], ref["pe"], rtol=1e-5, atol=1e-7)
-        check_fv(part, ref)
-    again, _ = compute(eng, kind, path, s, pot=pot)
-    for k in ("pe", "force", "virial"):
-        assert np.array_equal(again[k], out[k]), k
