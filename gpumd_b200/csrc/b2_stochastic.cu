@@ -12,8 +12,12 @@
 // The per-atom generator is cuRAND's XORWOW exactly as the reference uses it -- curand_init(seed, n, 0)
 // and three curand_normal_double draws per atom per call -- so a run seeded like the reference
 // (its -DDEBUG build passes glibc's first rand() = 1804289383) follows the reference's noise stream
-// draw for draw.  The momentum sums are one fused deterministic reduction (the block stage and ticket
-// of b2_reduce.cuh) instead of the reference's <<<4,1024>>> strided loops.
+// draw for draw.  That stream is pinned: tests/curand_oracle.py restates XORWOW (equal bit for bit to
+// cuRAND built for the host), and tests/test_gpu_langevin_steps.py holds these kernels, heat_lan's and
+// the driver's seeding to it, x, y, z per atom, the second Box-Muller value carried across calls, 64-bit
+// seeds and padded layouts included (within a few ulp: the device's sincospi is not the host's sin).
+// The momentum sums are one fused deterministic reduction (the block stage and ticket of b2_reduce.cuh)
+// instead of the reference's <<<4,1024>>> strided loops.
 #include "../../include/b200md.h"
 #include "b2_host.h"
 #include "b2_reduce.cuh"

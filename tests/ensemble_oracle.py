@@ -10,11 +10,13 @@ Group rules shared by every ensemble (src/integrate/ensemble.cu:111-174, 645-651
 """
 import numpy as np
 
+from curand_oracle import XorwowStates
 from oracle import oracle_py as O
 
 K_B = 8.617343e-5                    # src/utilities/common.cuh:21
 PRESSURE_UNIT_CONVERSION = 1.602177e+2  # src/utilities/common.cuh:25
-KINDS = ("nve", "nvt_ber", "nvt_nhc", "nvt_bdp", "npt_ber")
+KINDS = ("nve", "nvt_ber", "nvt_nhc", "nvt_bdp", "npt_ber", "nvt_lan", "nvt_bao")
+LANGEVIN_SEED = 1804289383  # glibc's first rand(): the seed of an unseeded run's first Langevin ensemble
 
 
 def pressure_parameters(target_pressure, elastic_modulus, tau_p):
@@ -35,7 +37,7 @@ class EnsembleStep:
 
     def __init__(self, kind, mass, time_step, pbc=(1, 1, 1), label=None, fixed_group=-1, move_group=-1,
                  move_velocity=(0.0, 0.0, 0.0), temperature=300.0, temperature_coupling=100.0,
-                 seed=12345678, target_pressure=None, elastic_modulus=None, tau_p=None):
+                 seed=None, target_pressure=None, elastic_modulus=None, tau_p=None):
         if kind not in KINDS:
             raise ValueError(kind)
         self.kind = kind
@@ -63,9 +65,14 @@ class EnsembleStep:
             self.ndeg = 3 * self.n_temperature
             if self.ndeg < 3:
                 raise ValueError("nvt_bdp needs at least one atom outside the fixed and moving groups")
-            self.bdp = O.BdpOracle(seed)
+            self.bdp = O.BdpOracle(12345678 if seed is None else seed)
         if kind == "npt_ber":
             self.num_p, self.p0, self.pc = pressure_parameters(target_pressure, elastic_modulus, tau_p)
+        if kind in ("nvt_lan", "nvt_bao"):
+            # ensemble_lan.cu:35-39 / ensemble_bao.cu:35-39: c1 = exp(-1/2 / tau) for the half kicks of
+            # nvt_lan, exp(-1 / tau) for nvt_bao's whole O step; curand_init(seed, i, 0) per atom
+            self.c1 = float(np.exp((-0.5 if kind == "nvt_lan" else -1.0) / self.temperature_coupling))
+            self.noise = XorwowStates(LANGEVIN_SEED if seed is None else seed, np.arange(n))
 
     # ---- the pieces
     def velocity_verlet(self, step1, pos, vel, force):
@@ -85,19 +92,46 @@ class EnsembleStep:
         factor = O.nhc_chain(self.chain, ek2, K_B * self.temperature, 3.0 * self.n, 0.5 * self.dt)
         return vel * factor
 
+    def langevin(self, vel):
+        """gpu_langevin + gpu_find_momentum + gpu_correct_momentum (langevin_utilities.cuh:26-127):
+        v <- c1 v + c2 / sqrt(m) xi on every atom, fixed ones included, with xi drawn x, y, z per atom and
+        c2 = sqrt((1 - c1^2) k_B T) from the target temperature of this kick; then the total momentum
+        (float64 sums) is removed."""
+        c2 = np.sqrt((1.0 - self.c1 * self.c1) * K_B * self.temperature)
+        xi = self.noise.normal_double(3)
+        v = self.c1 * vel + (c2 * np.sqrt(1.0 / self.mass))[None, :] * xi
+        return v - (v * self.mass).sum(axis=1, keepdims=True) / self.mass.sum()
+
+    def baoab(self, which, pos, vel, force):
+        """gpu_operator_A (which 0) / gpu_operator_B (which 1) with the fixed group frozen."""
+        return O.baoab_operator(which, self.dt, self.mass, pos, vel, force, self.label, self.fixed_group)
+
     # ---- the two halves around the force call
     def compute1(self, h, pos, vel, force):
         """Ensemble::compute1 up to the force call: (pos, vel)."""
+        if self.kind == "nvt_lan":  # ensemble_lan.cu:197-227: kick, then velocity-Verlet step 1
+            vel = self.langevin(vel)
+        if self.kind == "nvt_bao":  # ensemble_bao.cu:419-479: B A O A
+            pos, vel = self.baoab(1, pos, vel, force)
+            pos, vel = self.baoab(0, pos, vel, force)
+            vel = self.langevin(vel)
+            return self.baoab(0, pos, vel, force)
         if self.kind == "nvt_nhc":  # find_thermo, then the chain (ensemble_nhc.cu:184-195)
             vel = self.nhc_half(self.find_thermo(h, np.zeros(self.n), vel, np.zeros((9, self.n)))[0], vel)
         return self.velocity_verlet(True, pos, vel, force)
 
     def compute2(self, h, pos, vel, force, pe, virial):
         """Ensemble::compute2 after the force call: (pos, vel, h, thermo[8]).  thermo is the one
-        find_thermo leaves, before any thermostat or barostat acts on the state."""
+        find_thermo leaves: before any thermostat or barostat acts on the state, except for nvt_lan,
+        whose second kick comes before find_thermo."""
         h = np.array(h, dtype=np.float64).reshape(9)
         pos = np.array(pos, dtype=np.float64)
+        if self.kind == "nvt_bao":  # Ensemble_BAO::compute2, ensemble_bao.cu:481: B, then thermo
+            _, vel = self.baoab(1, pos, vel, force)
+            return pos, vel, h, self.find_thermo(h, pe, vel, virial)
         _, vel = self.velocity_verlet(False, pos, vel, force)
+        if self.kind == "nvt_lan":  # Ensemble_LAN::compute2, ensemble_lan.cu:229: step 2, kick, then thermo
+            vel = self.langevin(vel)
         thermo = self.find_thermo(h, pe, vel, virial)
         T, Tc = self.temperature, self.temperature_coupling
         if self.kind in ("nvt_ber", "npt_ber"):  # Ensemble_BER::compute2, ensemble_ber.cu:195-233

@@ -93,6 +93,38 @@ def nhc_energy(state, ek2, dof, kT):
     return 0.5 * ek2 + (0.5 * ve * ve / Q).sum() + dof * kT * eta[0] + kT * eta[1:].sum()
 
 
+class HeatLan:
+    """heat_lan's bath (Ensemble_LAN heat branch, ensemble_lan.cu:43-85,128-195, with the groups' gpu_langevin
+    of langevin_utilities.cuh:127-149): two XORWOW streams, curand_init(seed_source, m, 0) for the m-th
+    source atom and curand_init(seed_sink, m, 0) for the m-th sink atom, m the position within the group
+    in `contents` order.  Each half kicks v <- c1 v + c2_g / sqrt(m) xi on the source then the sink
+    (c1 = exp(-1/2 / Tc), c2_g = sqrt((1 - c1^2) k_B (T +- dT))), with no momentum correction, and adds
+    1/2 sum m (v_before^2 - v_after^2) to the group's energy.  Other atoms are untouched."""
+
+    def __init__(self, mass, label, source, sink, T, Tc, dT, seed_source, seed_sink):
+        from curand_oracle import XorwowStates
+        self.mass = np.asarray(mass, dtype=np.float64)
+        sizes, order = contents(label)
+        start = np.concatenate([[0], np.cumsum(sizes)])
+        self.atoms = [order[start[g]:start[g + 1]] for g in (source, sink)]
+        self.c1 = float(np.exp(-0.5 / Tc))
+        self.c2 = [float(np.sqrt((1.0 - self.c1 * self.c1) * K_B * t)) for t in (T + dT, T - dT)]
+        self.noise = [XorwowStates(seed, np.arange(idx.shape[0]))
+                      for seed, idx in zip((seed_source, seed_sink), self.atoms)]
+        self.energy = np.zeros(2)
+
+    def half(self, vel):
+        v = np.array(vel, dtype=np.float64)
+        for g in range(2):
+            idx = self.atoms[g]
+            m = self.mass[idx]
+            v0 = v[:, idx]
+            v1 = self.c1 * v0 + (self.c2[g] * np.sqrt(1.0 / m))[None, :] * self.noise[g].normal_double(3)
+            v[:, idx] = v1
+            self.energy[g] += (0.5 * m * (v0 * v0 - v1 * v1).sum(axis=0)).sum()
+        return v
+
+
 def bdp_factors(mt, mass, vel, src, snk, T, dT, Tc):
     """integrate_heat_bdp_2 (ensemble_bdp.cu:103-149): factors and energies of source then sink; mt is a
     BdpOracle (one stream for both groups)."""

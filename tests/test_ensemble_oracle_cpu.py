@@ -195,3 +195,80 @@ def test_bdp_stream_depends_on_the_degrees_of_freedom(oracle, n_atoms, k):
         assert [c for _, c in a[1:]] != [c for _, c in b[1:]]
     if 3 * n_atoms <= 12:
         assert a[0][1] != b[0][1]
+
+
+# ---------------------------------------------------------------- nvt_lan / nvt_bao
+
+def zero_momentum_state(n=256, seed=11):
+    """Atom i + n/2 is atom i, in the same group, with the velocity and forces negated: the momentum of each half is the exact
+    negative of the other's after any step, and numpy's pairwise sum splits 256 atoms into these two
+    halves, so the total momentum is exactly zero."""
+    s = random_state(n=n, seed=seed)
+    half = n // 2
+    s["mass"] = np.concatenate([s["mass"][:half]] * 2)
+    s["label"] = np.concatenate([s["label"][:half]] * 2)
+    for k in ("vel", "f0", "f1"):
+        s[k] = np.concatenate([s[k][:, :half], -s[k][:, :half]], axis=1)
+    return s
+
+
+@pytest.mark.parametrize("groups", ["none", "fix"])
+def test_langevin_without_friction_or_noise_is_nve(groups):
+    """c1 = 1 (infinite coupling time) and c2 = 0 leave a kick v <- c1 v + c2 / sqrt(m) xi and the
+    momentum removal with nothing to do on a state of zero total momentum: nvt_lan is then nve bit for
+    bit, and nvt_bao (B A A | force | B) is nve up to the rounding of two half drifts instead of one."""
+    s = zero_momentum_state()
+    g = GROUPS[groups]
+    label = s["label"] if g else None
+    nve = EnsembleStep("nve", s["mass"], DT, label=label, **g)
+    want = nve.step(s["h"], s["pos"], s["vel"], s["f0"], s["f1"], s["pe"], s["vir"])
+    for kind in ("nvt_lan", "nvt_bao"):
+        e = EnsembleStep(kind, s["mass"], DT, label=label, temperature=300.0, temperature_coupling=np.inf, **g)
+        assert e.c1 == 1.0
+        got = e.step(s["h"], s["pos"], s["vel"], s["f0"], s["f1"], s["pe"], s["vir"])
+        for a, b, what in zip(got, want, ("pos", "vel", "h", "thermo")):
+            if kind == "nvt_lan" or what == "h":
+                assert np.array_equal(a, b), (kind, what)
+            else:
+                assert np.allclose(a, b, rtol=1e-14, atol=1e-14 * np.abs(b).max()), (kind, what)
+
+
+@pytest.mark.parametrize("kind", ["nvt_lan", "nvt_bao"])
+def test_langevin_kick_removes_the_momentum_and_draws_per_atom(kind):
+    """After every kick the total momentum is zero to rounding; the noise of atom i is normal number
+    3c..3c+2 of curand_init(seed, i, 0), x then y then z, on every atom whatever its group."""
+    import curand_oracle as X
+    s = random_state(seed=9)
+    e = EnsembleStep(kind, s["mass"], DT, label=s["label"], fixed_group=1, temperature=300.0,
+                     temperature_coupling=20.0)
+    v = s["vel"]
+    stream = X.XorwowStates(1804289383, np.arange(len(s["mass"])))
+    c2 = np.sqrt((1 - e.c1 ** 2) * K_B * 300.0)
+    for _ in range(4):
+        xi = stream.normal_double(3)
+        raw = e.c1 * v + c2 * np.sqrt(1.0 / s["mass"]) * xi
+        v = e.langevin(v)
+        p = (v * s["mass"]).sum(axis=1)
+        assert np.abs(p).max() < 1e-13 * (np.abs(v) * s["mass"]).sum()
+        shift = raw - v  # one momentum shift for all atoms
+        assert np.allclose(shift, shift[:, :1], rtol=0, atol=1e-15)
+
+
+@pytest.mark.parametrize("kind", ["nvt_lan", "nvt_bao"])
+def test_langevin_fixed_atom_rules(kind):
+    """Fixed atoms keep their position bit for bit.  nvt_bao's B step leaves their velocity at zero at
+    the end of each step; nvt_lan's last kick draws noise for them too (the reference kicks every atom)."""
+    s = random_state(seed=4)
+    e = EnsembleStep(kind, s["mass"], DT, label=s["label"], fixed_group=2, temperature=300.0,
+                     temperature_coupling=30.0)
+    fixed = s["label"] == 2
+    h, pos, vel = s["h"], s["pos"], s["vel"]
+    for k in range(3):
+        p1, v1 = e.compute1(h, pos, vel, s["f0"])
+        assert np.array_equal(p1[:, fixed], pos[:, fixed]), k
+        pos, vel, h, th = e.compute2(h, p1, v1, s["f1"], s["pe"], s["vir"])
+        assert np.array_equal(pos[:, fixed], p1[:, fixed])
+        if kind == "nvt_bao":
+            assert np.all(vel[:, fixed] == 0.0)
+        else:
+            assert np.all(vel[:, fixed] != 0.0)

@@ -64,3 +64,41 @@ def test_resamplekin_stream_is_reproducible_and_unbiased():
     c = no.BdpOracle(1)
     draws = np.array([c.resamplekin(100.0, 120.0, 30, 0.0) for _ in range(4000)])
     assert abs(draws.mean() - 120.0) < 4 * 120.0 * np.sqrt(2 / 30 / 4000)
+
+
+def heat_lan_setup(n=500, seed=3):
+    rng = np.random.default_rng(seed)
+    mass = rng.uniform(1.0, 200.0, n)
+    label = rng.integers(0, 5, n).astype(np.int32)  # interleaved: the group contents are not contiguous
+    vel = rng.normal(size=(3, n)) * 0.01
+    return mass, label, vel
+
+
+def test_heat_lan_kicks_only_source_and_sink_and_accounts_the_energy():
+    import curand_oracle as X
+    mass, label, vel = heat_lan_setup()
+    bath = no.HeatLan(mass, label, 1, 3, 300.0, 10.0, 30.0, 1804289383, 846930886)
+    sizes, order = no.contents(label)
+    src, snk = order[label[order] == 1], order[label[order] == 3]
+    assert np.array_equal(bath.atoms[0], src) and np.array_equal(bath.atoms[1], snk)
+    streams = [X.XorwowStates(1804289383, np.arange(sizes[1])), X.XorwowStates(846930886, np.arange(sizes[3]))]
+    v = vel
+    energy = np.zeros(2)
+    for _ in range(5):
+        v1 = bath.half(v)
+        other = (label != 1) & (label != 3)
+        assert np.array_equal(v1[:, other], v[:, other])
+        for g, (idx, T) in enumerate(((src, 330.0), (snk, 270.0))):
+            c2 = np.sqrt((1 - bath.c1 ** 2) * no.K_B * T)
+            want = bath.c1 * v[:, idx] + c2 * np.sqrt(1.0 / mass[idx]) * streams[g].normal_double(3)
+            assert np.array_equal(v1[:, idx], want)
+            energy[g] += 0.5 * (mass[idx] * ((v[:, idx] ** 2).sum(0) - (want ** 2).sum(0))).sum()
+        v = v1
+    assert np.allclose(bath.energy, energy, rtol=1e-13, atol=0)
+
+
+def test_heat_lan_without_friction_or_noise_changes_nothing():
+    mass, label, vel = heat_lan_setup(seed=4)
+    bath = no.HeatLan(mass, label, 0, 4, 300.0, np.inf, 10.0, 1, 2)
+    assert bath.c1 == 1.0 and bath.c2 == [0.0, 0.0]
+    assert np.array_equal(bath.half(vel), vel) and np.all(bath.energy == 0.0)
