@@ -75,10 +75,12 @@ __global__ void __launch_bounds__(256) k_hnemd_correct(
 }
 
 // compute_heat + gpu_sum_heat of hnemd_kappa.cu:52-106 in one pass: the per-atom heat current is
-// summed straight into row5[0..4]; the 5N per-atom array is never written
+// summed straight into a row of five; the 5N per-atom array is never written.  row_at == nullptr: the
+// row is rows[0..4]; otherwise it is row *row_at of rows[n_rows][5], and the last block advances
+// *row_at (mod n_rows), so that one captured launch serves every step
 __global__ void __launch_bounds__(RED_BLK) k_hnemd_heat(
-  int n, int stride, const double* __restrict__ w, const double* __restrict__ v, double* row5,
-  double* partial, unsigned int* ticket)
+  int n, int stride, const double* __restrict__ w, const double* __restrict__ v, double* rows,
+  unsigned int* row_at, unsigned int n_rows, double* partial, unsigned int* ticket)
 {
   double t[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -89,8 +91,12 @@ __global__ void __launch_bounds__(RED_BLK) k_hnemd_heat(
       t[k] += h[k];
   }
   b2_block_totals<5, RED_BLK>(t, partial + blockIdx.x, gridDim.x);
-  if (b2_last_block(ticket))
+  if (b2_last_block(ticket)) {
+    double* row5 = row_at ? rows + (size_t)5 * *row_at : rows;
     b2_grid_totals<5, RED_BLK>(partial, [&](int k, double v) { row5[k] = v; });
+    if (row_at && threadIdx.x == 0) // after the barrier that ends b2_grid_totals: every put has read it
+      *row_at = (*row_at + 1u) % n_rows;
+  }
 }
 
 // one block per heat component: strided partial sums, then a tree -- the order of hac.cu:50-78
@@ -138,6 +144,30 @@ __global__ void __launch_bounds__(128) k_find_hac(int Nc, int Nd, const double* 
   if (tid == 0)
     for (int k = 0; k < 5; ++k)
       g_hac[bid + (size_t)Nc * k] = s[k][0] / (Nd - bid);
+}
+
+// |fe| as HNEMD::parse forms it, hnemd_kappa.cu:180-183
+double fe_norm(const double fe[3])
+{
+  double norm = 0.0;
+  for (int d = 0; d < 3; ++d)
+    norm += fe[d] * fe[d];
+  return std::sqrt(norm);
+}
+
+// the output branch of HNEMD::process, hnemd_kappa.cu:108-122: rows[m * 5 + k], m < oi, summed in
+// order and scaled to W/mK
+void hnemd_kappa(int oi, double volume, double temperature, double fe_norm, const double* rows, double* kappa5)
+{
+  const double KAPPA_UNIT_CONVERSION = 1.573769e+5; // common.cuh:27
+  double factor = KAPPA_UNIT_CONVERSION / oi;
+  factor /= (volume * temperature * fe_norm);
+  for (int k = 0; k < 5; ++k) {
+    double s = 0.0;
+    for (int m = 0; m < oi; ++m)
+      s += rows[(size_t)m * 5 + k];
+    kappa5[k] = s * factor;
+  }
 }
 
 } // namespace
@@ -247,6 +277,37 @@ long long b200md_hnemd_drive_scratch_bytes(int n)
   return (long long)(b2_scratch_bytes(3, b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS)) + sizeof(double) * FTOT_SLOT);
 }
 
+int b200md_hnemd_drive_add(
+  int n, int stride, const double fe[3], const double* d_virial, double* d_force, void* d_scratch,
+  double* d_ftot, void* stream)
+{
+  if (n < 0 || stride < n || !fe || (n > 0 && (!d_virial || !d_force)) || !d_scratch || !d_ftot) {
+    set_error("b200md_hnemd_drive_add: bad argument");
+    return B200MD_ERR_ARG;
+  }
+  // the partials sit behind the FTOT_SLOT of b200md_hnemd_drive's layout; n = 0 is one block that
+  // writes a zero total
+  k_hnemd_drive<<<b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS), RED_BLK, 0, (cudaStream_t)stream>>>(
+    n, stride, fe[0], fe[1], fe[2], d_virial, d_force, b2_scratch_partials(d_scratch) + FTOT_SLOT,
+    b2_scratch_ticket(d_scratch), d_ftot);
+  B2_LAUNCHED();
+  return B200MD_OK;
+}
+
+int b200md_hnemd_drive_correct(
+  int n, int stride, double one_over_n, const double* d_ftot, double* d_force, void* stream)
+{
+  if (n < 0 || stride < n || !d_ftot || (n > 0 && !d_force)) {
+    set_error("b200md_hnemd_drive_correct: bad argument");
+    return B200MD_ERR_ARG;
+  }
+  if (n == 0) // a zero-block grid is a launch error
+    return B200MD_OK;
+  k_hnemd_correct<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(n, stride, one_over_n, d_ftot, d_force);
+  B2_LAUNCHED();
+  return B200MD_OK;
+}
+
 int b200md_hnemd_drive(
   int n, int stride, const double fe[3], const double* d_virial, double* d_force, void* d_scratch,
   void* stream)
@@ -257,11 +318,29 @@ int b200md_hnemd_drive(
   }
   // the b2_scratch_* layout with ftot[3] in front of the partials
   double* ftot = b2_scratch_partials(d_scratch);
-  cudaStream_t st = (cudaStream_t)stream;
-  k_hnemd_drive<<<b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS), RED_BLK, 0, st>>>(
-    n, stride, fe[0], fe[1], fe[2], d_virial, d_force, ftot + FTOT_SLOT, b2_scratch_ticket(d_scratch), ftot);
-  B2_LAUNCHED();
-  k_hnemd_correct<<<grid_for(n, 256), 256, 0, st>>>(n, stride, 1.0 / n, ftot, d_force);
+  const int rc = b200md_hnemd_drive_add(n, stride, fe, d_virial, d_force, d_scratch, ftot, stream);
+  if (rc != B200MD_OK)
+    return rc;
+  return b200md_hnemd_drive_correct(n, stride, 1.0 / n, ftot, d_force, stream);
+}
+
+long long b200md_hnemd_heat_row_scratch_bytes(int n)
+{
+  return (long long)b2_scratch_bytes(5, b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS));
+}
+
+int b200md_hnemd_heat_row(
+  int n, int stride, const double* d_virial, const double* d_velocity, double* d_rows, int n_rows,
+  unsigned int* d_row, void* d_scratch, void* stream)
+{
+  if (n < 0 || stride < n || n_rows < 1 || (n > 0 && (!d_virial || !d_velocity)) || !d_rows || !d_row ||
+      !d_scratch) {
+    set_error("b200md_hnemd_heat_row: bad argument");
+    return B200MD_ERR_ARG;
+  }
+  k_hnemd_heat<<<b2_reduce_blocks(n, RED_BLK, RED_MAX_BLOCKS), RED_BLK, 0, (cudaStream_t)stream>>>(
+    n, stride, d_virial, d_velocity, d_rows, d_row, (unsigned int)n_rows, b2_scratch_partials(d_scratch),
+    b2_scratch_ticket(d_scratch));
   B2_LAUNCHED();
   return B200MD_OK;
 }
@@ -278,12 +357,9 @@ int b200md_hnemd_create(int output_interval, const double fe[3], b200md_hnemd** 
     return B200MD_ERR_ARG;
   }
   p->output_interval = output_interval;
-  double norm = 0.0;
-  for (int d = 0; d < 3; ++d) {
+  for (int d = 0; d < 3; ++d)
     p->fe[d] = fe[d];
-    norm += fe[d] * fe[d]; // hnemd_kappa.cu:180-183
-  }
-  p->fe_norm = std::sqrt(norm);
+  p->fe_norm = fe_norm(fe);
   if (p->heat_all.reserve((size_t)5 * output_interval) != cudaSuccess) {
     delete p;
     set_error("out of device memory (HNEMD)");
@@ -312,8 +388,8 @@ int b200md_hnemd_sample(
   }
   const int row = step % p->output_interval;
   k_hnemd_heat<<<g, RED_BLK, 0, (cudaStream_t)stream>>>(
-    n, stride, d_virial, d_velocity, p->heat_all.p + (size_t)5 * row, b2_scratch_partials(p->scratch.p),
-    b2_scratch_ticket(p->scratch.p));
+    n, stride, d_virial, d_velocity, p->heat_all.p + (size_t)5 * row, nullptr, 0u,
+    b2_scratch_partials(p->scratch.p), b2_scratch_ticket(p->scratch.p));
   B2_LAUNCHED();
   return B200MD_OK;
 }
@@ -330,18 +406,23 @@ int b200md_hnemd_take(
   cudaStream_t st = (cudaStream_t)stream;
   B2_CUDA(cudaMemcpyAsync(h.data(), p->heat_all.p, sizeof(double) * 5 * oi, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
-  const double KAPPA_UNIT_CONVERSION = 1.573769e+5; // common.cuh:27
-  double factor = KAPPA_UNIT_CONVERSION / oi;         // hnemd_kappa.cu:112-122
-  factor /= (volume * temperature * p->fe_norm);
-  for (int k = 0; k < 5; ++k) {
-    double s = 0.0;
-    for (int m = 0; m < oi; ++m)
-      s += h[(size_t)m * 5 + k];
-    kappa5[k] = s * factor;
-  }
+  hnemd_kappa(oi, volume, temperature, p->fe_norm, h.data(), kappa5);
   if (rows)
     for (size_t k = 0; k < h.size(); ++k)
       rows[k] = h[k];
+  return B200MD_OK;
+}
+
+int b200md_hnemd_kappa(
+  int output_interval, double volume, double temperature, const double fe[3], const double* rows,
+  double* kappa5)
+{
+  if (output_interval < 1 || !fe || !rows || !kappa5 || !(volume > 0.0) || !(temperature > 0.0) ||
+      !(fe_norm(fe) > 0.0)) {
+    set_error("b200md_hnemd_kappa: need output_interval >= 1, volume > 0, temperature > 0 and |fe| > 0");
+    return B200MD_ERR_ARG;
+  }
+  hnemd_kappa(output_interval, volume, temperature, fe_norm(fe), rows, kappa5);
   return B200MD_OK;
 }
 

@@ -18,6 +18,8 @@
 #include <cuda_runtime.h>
 #include <nccl.h>
 
+#include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -349,6 +351,11 @@ struct Domain {
   DBuf<unsigned char> thermo_scratch;
   DBuf<double> heat, heat5;
   DBuf<unsigned int> disp_bits;
+  // HNEMD: this block's total of the driven forces (then the global one), its heat-current rows and
+  // the ring row the next one goes to, and the scratch of both reductions
+  DBuf<double> hn_ftot, hn_rows;
+  DBuf<unsigned int> hn_row;
+  DBuf<unsigned char> hn_scratch;
   ~Domain()
   {
     if (nhc)
@@ -372,7 +379,14 @@ struct b200md_mgpu {
   long long n_global = 0;
   int migrations = 0;
   int steps_since_exchange = 0;
-  DBuf<double> thermo_sum;
+  DBuf<double> thermo_sum; // local mode: the domains' sums of thermo[8] or of the HNEMD force total
+  // HNEMD (b200md_mgpu_hnemd_set): each domain's heat rows form a ring of hn_ring rows; the hn_pending
+  // steps sampled since the last take start at ring row hn_first
+  bool hn_on = false;
+  double hn_fe[3] = {0, 0, 0};
+  int hn_oi = 1, hn_max = 0, hn_ring = 0, hn_first = 0;
+  long long hn_pending = 0;
+  DBuf<double> hn_gather; // distributed: every rank's ring, gathered at take time
   DBuf<int> cnt_dev;
   // profiling
   bool prof = false;
@@ -814,26 +828,65 @@ int compute_force(Group& G)
   return B200MD_OK;
 }
 
+// the sum over all domains of (D.*buf)[0..n), n <= 8, lands in every domain's buffer: one
+// ncclAllReduce, or in local mode a sum in domain order
+int sum_over_domains(Group& G, DBuf<double> Domain::*buf, int n)
+{
+  cudaStream_t st = G.stream;
+  if (G.distributed) {
+    double* p = ((*G.dom[0]).*buf).p;
+    MG_NCCL(ncclAllReduce(p, p, n, ncclDouble, ncclSum, G.comm, st));
+  } else if (G.dom.size() > 1) {
+    MG_CUDA(cudaMemsetAsync(G.thermo_sum.p, 0, n * sizeof(double), st));
+    for (auto& dp : G.dom)
+      k_add8<<<1, 32, 0, st>>>(G.thermo_sum.p, ((*dp).*buf).p, n); MG_COUNT();
+    for (auto& dp : G.dom)
+      MG_CUDA(cudaMemcpyAsync(((*dp).*buf).p, G.thermo_sum.p, n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  }
+  return B200MD_OK;
+}
+
 // partial sums over the owned atoms, then the global sum lands in every domain's thermo[]; a block
 // that owns no atoms still runs it, because its single thread block writes the zero partial
 int find_thermo(Group& G)
 {
-  cudaStream_t st = G.stream;
   for (auto& dp : G.dom) {
     Domain& D = *dp;
     MG_B2(b200md_find_thermo_strided(
       D.n_own, D.n_loc, (int)G.n_global, G.volume, D.mass.p, D.pe.p, D.vel.p, D.virial.p, D.thermo.p,
-      D.thermo_scratch.p, st));
+      D.thermo_scratch.p, G.stream));
   }
-  if (G.distributed) {
-    Domain& D = *G.dom[0];
-    MG_NCCL(ncclAllReduce(D.thermo.p, D.thermo.p, 8, ncclDouble, ncclSum, G.comm, st));
-  } else if (G.dom.size() > 1) {
-    MG_CUDA(cudaMemsetAsync(G.thermo_sum.p, 0, 8 * sizeof(double), st));
-    for (auto& dp : G.dom)
-      k_add8<<<1, 32, 0, st>>>(G.thermo_sum.p, dp->thermo.p, 8); MG_COUNT();
-    for (auto& dp : G.dom)
-      MG_CUDA(cudaMemcpyAsync(dp->thermo.p, G.thermo_sum.p, 8 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  return sum_over_domains(G, &Domain::thermo, 8);
+}
+
+// compute_hnemd's drive (force.cu:857-897) on the blocks: f_i += W_i^T fe on the owned atoms with each
+// block's total of the new forces, the global total, then f_i -= total / N.  A block that owns no
+// atoms contributes the zero total of its single thread block and skips the correction.
+int hnemd_drive(Group& G)
+{
+  cudaStream_t st = G.stream;
+  for (auto& dp : G.dom) {
+    Domain& D = *dp;
+    MG_B2(b200md_hnemd_drive_add(
+      D.n_own, D.n_loc, G.hn_fe, D.virial.p, D.force.p, D.hn_scratch.p, D.hn_ftot.p, st));
+  }
+  MG_TRY(sum_over_domains(G, &Domain::hn_ftot, 3));
+  const double one_over_n = 1.0 / (double)G.n_global;
+  for (auto& dp : G.dom) {
+    Domain& D = *dp;
+    MG_B2(b200md_hnemd_drive_correct(D.n_own, D.n_loc, one_over_n, D.hn_ftot.p, D.force.p, st));
+  }
+  return B200MD_OK;
+}
+
+// HNEMD::process (hnemd_kappa.cu:82-106) on the blocks: every block sums the heat current of its owned
+// atoms into its own ring row; blocks are summed only at take time
+int hnemd_heat(Group& G)
+{
+  for (auto& dp : G.dom) {
+    Domain& D = *dp;
+    MG_B2(b200md_hnemd_heat_row(
+      D.n_own, D.n_loc, D.virial.p, D.vel.p, D.hn_rows.p, G.hn_ring, D.hn_row.p, D.hn_scratch.p, G.stream));
   }
   return B200MD_OK;
 }
@@ -883,6 +936,8 @@ int one_step(Group& G, double dt)
   MG_TRY(halo_update(G));
   mark(G, 2);
   MG_TRY(compute_force(G));
+  if (G.hn_on)
+    MG_TRY(hnemd_drive(G));
   mark(G, 3);
   for (auto& dp : G.dom) {
     Domain& D = *dp;
@@ -903,6 +958,8 @@ int one_step(Group& G, double dt)
         MG_B2(b200md_bdp_step(D.bdp, D.n_own, D.n_loc, D.thermo.p, D.vel.p, st));
     }
   }
+  if (G.hn_on)
+    MG_TRY(hnemd_heat(G));
   mark(G, 4);
   return B200MD_OK;
 }
@@ -1054,6 +1111,7 @@ int b200md_mgpu_distribute(
   Group& G = *g;
   cudaStream_t st = G.stream;
   G.n_global = n_global;
+  G.hn_on = false; // the domains' buffers are about to be re-sized: b200md_mgpu_hnemd_set comes after
   const size_t N = (size_t)n_global;
   // owner of every atom from its wrapped coordinate
   std::vector<int> owner(N);
@@ -1170,6 +1228,14 @@ int b200md_mgpu_run(b200md_mgpu* g, int nsteps, int check_every)
   const double dt = G.cfg.time_step;
   if (check_every < 1)
     check_every = 5;
+  if (G.hn_on && nsteps > 0 && (G.hn_pending + nsteps) / G.hn_oi > G.hn_max)
+    return fail(B200MD_ERR_OVERFLOW, "b200md_mgpu_run: the run would complete more HNEMD intervals than "
+                                     "max_intervals before the next b200md_mgpu_hnemd_take");
+  auto stepped = [&G] { // every step enqueued writes one HNEMD heat row
+    ++G.steps_since_exchange;
+    if (G.hn_on)
+      ++G.hn_pending;
+  };
   for (int s = 0; s < nsteps; ++s) {
     if (G.steps_since_exchange && G.steps_since_exchange % check_every == 0) {
       bool need = false;
@@ -1185,7 +1251,7 @@ int b200md_mgpu_run(b200md_mgpu* g, int nsteps, int check_every)
         }
         // one eager step first so that nothing allocates or synchronises inside the capture
         MG_TRY(one_step(G, dt));
-        ++G.steps_since_exchange;
+        stepped();
         if (++s >= nsteps)
           break;
         cudaGraph_t graph = nullptr;
@@ -1212,7 +1278,7 @@ int b200md_mgpu_run(b200md_mgpu* g, int nsteps, int check_every)
         ++G.prof_steps;
       }
     }
-    ++G.steps_since_exchange;
+    stepped();
   }
   return B200MD_OK;
 }
@@ -1280,6 +1346,106 @@ int b200md_mgpu_heat_current(b200md_mgpu* g, double out5[5])
   }
   for (int k = 0; k < 5; ++k)
     out5[k] = tot[k];
+  return B200MD_OK;
+}
+
+int b200md_mgpu_hnemd_set(b200md_mgpu* g, int output_interval, const double fe[3], int max_intervals)
+{
+  if (!g || !fe || output_interval < 1 || max_intervals < 1)
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_set: need output_interval >= 1, max_intervals >= 1 and fe[3]");
+  if (!std::isfinite(fe[0]) || !std::isfinite(fe[1]) || !std::isfinite(fe[2]))
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_set: fe must be finite");
+  if ((long long)(max_intervals + 1LL) * output_interval > INT_MAX / 5)
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_set: (max_intervals + 1) * output_interval rows are too many");
+  Group& G = *g;
+  if (G.n_global <= 0)
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_set: call b200md_mgpu_distribute first");
+  cudaStream_t st = G.stream;
+  MG_CUDA(cudaStreamSynchronize(st)); // buffers of a previous setting may still be in use
+  if (G.graph) { // the step gains or loses launches
+    cudaGraphExecDestroy(G.graph);
+    G.graph = nullptr;
+  }
+  G.hn_on = fe[0] != 0.0 || fe[1] != 0.0 || fe[2] != 0.0; // fe = 0: Force::finalize, force.cu:335-339
+  for (int d = 0; d < 3; ++d)
+    G.hn_fe[d] = fe[d];
+  G.hn_oi = output_interval;
+  G.hn_max = max_intervals;
+  // a take finds at most max_intervals whole intervals and a partial one
+  G.hn_ring = (max_intervals + 1) * output_interval;
+  G.hn_first = 0;
+  G.hn_pending = 0;
+  if (G.hn_on) {
+    const size_t ring = (size_t)5 * G.hn_ring;
+    for (auto& dp : G.dom) {
+      Domain& D = *dp;
+      const size_t sb = (size_t)std::max(b200md_hnemd_drive_scratch_bytes(D.cap),
+                                         b200md_hnemd_heat_row_scratch_bytes(D.cap));
+      MG_CUDA(D.hn_ftot.reserve(3));
+      MG_CUDA(D.hn_rows.reserve(ring));
+      MG_CUDA(D.hn_row.reserve(1));
+      MG_CUDA(D.hn_scratch.reserve(sb));
+      MG_CUDA(cudaMemsetAsync(D.hn_rows.p, 0, sizeof(double) * ring, st));
+      MG_CUDA(cudaMemsetAsync(D.hn_row.p, 0, sizeof(unsigned int), st));
+      MG_CUDA(cudaMemsetAsync(D.hn_scratch.p, 0, sb, st));
+    }
+    if (G.distributed)
+      MG_CUDA(G.hn_gather.reserve(ring * G.world));
+  }
+  // forces at the current positions as the next step's first half expects them (the evaluation before
+  // a run's loop, run.cu:217-248); the ghosts' positions are those of the last force call
+  MG_TRY(compute_force(G));
+  if (G.hn_on)
+    MG_TRY(hnemd_drive(G));
+  MG_CUDA(cudaStreamSynchronize(st));
+  return b200md_mgpu_check(g);
+}
+
+int b200md_mgpu_hnemd_take(b200md_mgpu* g, double temperature, int* n_intervals, double* kappa, double* rows)
+{
+  if (!g || !n_intervals || !kappa || !(temperature > 0.0))
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_take: need temperature > 0, n_intervals and kappa");
+  Group& G = *g;
+  if (!G.hn_on)
+    return fail(B200MD_ERR_ARG, "b200md_mgpu_hnemd_take: HNEMD is off (b200md_mgpu_hnemd_set with fe != 0)");
+  cudaStream_t st = G.stream;
+  const int oi = G.hn_oi, m = (int)(G.hn_pending / oi);
+  const size_t ring = (size_t)5 * G.hn_ring;
+  // the rows of all blocks, summed in block (= rank) order on the host
+  std::vector<double> all, sum(ring);
+  if (G.distributed) {
+    Domain& D = *G.dom[0];
+    all.resize(ring * G.world);
+    MG_NCCL(ncclAllGather(D.hn_rows.p, G.hn_gather.p, ring, ncclDouble, G.comm, st));
+    MG_CUDA(cudaMemcpyAsync(all.data(), G.hn_gather.p, sizeof(double) * all.size(), cudaMemcpyDeviceToHost, st));
+  } else {
+    all.resize(ring * G.dom.size());
+    for (size_t k = 0; k < G.dom.size(); ++k)
+      MG_CUDA(cudaMemcpyAsync(all.data() + ring * k, G.dom[k]->hn_rows.p, sizeof(double) * ring,
+                              cudaMemcpyDeviceToHost, st));
+  }
+  MG_CUDA(cudaStreamSynchronize(st));
+  const size_t blocks = all.size() / ring;
+  for (size_t e = 0; e < ring; ++e) {
+    double v = all[e];
+    for (size_t k = 1; k < blocks; ++k)
+      v += all[ring * k + e];
+    sum[e] = v;
+  }
+  std::vector<double> h((size_t)5 * oi);
+  for (int j = 0; j < m; ++j) {
+    for (int r = 0; r < oi; ++r) {
+      const size_t at = (size_t)((G.hn_first + (long long)j * oi + r) % G.hn_ring);
+      for (int k = 0; k < 5; ++k)
+        h[(size_t)5 * r + k] = sum[5 * at + k];
+    }
+    MG_B2(b200md_hnemd_kappa(oi, G.volume, temperature, G.hn_fe, h.data(), kappa + (size_t)5 * j));
+    if (rows)
+      std::copy(h.begin(), h.end(), rows + (size_t)5 * oi * j);
+  }
+  G.hn_first = (int)((G.hn_first + (long long)m * oi) % G.hn_ring);
+  G.hn_pending -= (long long)m * oi;
+  *n_intervals = m;
   return B200MD_OK;
 }
 

@@ -89,6 +89,11 @@ SIGNATURES = {
     "b200md_hnemd_destroy": (None, [_vp]),
     "b200md_hnemd_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),
     "b200md_hnemd_take": (C.c_int, [_vp, C.c_double, C.c_double, _dp, _dp, _vp]),
+    "b200md_hnemd_drive_add": (C.c_int, [C.c_int, C.c_int, _dp, _vp, _vp, _vp, _vp, _vp]),
+    "b200md_hnemd_drive_correct": (C.c_int, [C.c_int, C.c_int, C.c_double, _vp, _vp, _vp]),
+    "b200md_hnemd_heat_row_scratch_bytes": (C.c_longlong, [C.c_int]),
+    "b200md_hnemd_heat_row": (C.c_int, [C.c_int, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp]),
+    "b200md_hnemd_kappa": (C.c_int, [C.c_int, C.c_double, C.c_double, _dp, _dp, _dp]),
     "b200md_shc_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _ip, _ip, C.POINTER(_vp)]),
     "b200md_shc_destroy": (None, [_vp]),
     "b200md_shc_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp]),

@@ -51,6 +51,8 @@ def load():
         L.b200md_mgpu_get_local.argtypes = [vp, C.c_int, vp, vp, dp, C.POINTER(C.c_int)]
         L.b200md_mgpu_profile.argtypes = [vp, C.c_int, dp, C.c_int]
         L.b200md_mgpu_check.argtypes = [vp]
+        L.b200md_mgpu_hnemd_set.argtypes = [vp, C.c_int, dp, C.c_int]
+        L.b200md_mgpu_hnemd_take.argtypes = [vp, C.c_double, C.POINTER(C.c_int), dp, dp]
         _LIB = L
     return _LIB
 
@@ -136,6 +138,27 @@ class DomainGroup:
         out = (C.c_double * 5)()
         _check(self._L.b200md_mgpu_heat_current(self._h, out))
         return np.array(out[:])
+
+    _hnemd = (1, 1)  # (output_interval, max_intervals) of the last set_hnemd: the sizes of a take
+
+    def set_hnemd(self, output_interval, fe, max_intervals=100):
+        """compute_hnemd inside the step (after distribute): fe (3 floats, 1/A) drives every step, a heat
+        row is summed every step and hnemd_take() returns the finished intervals.  fe = 0 switches it
+        off.  A run that would leave more than max_intervals intervals untaken is refused."""
+        fe3 = (C.c_double * 3)(*[float(x) for x in fe])
+        _check(self._L.b200md_mgpu_hnemd_set(self._h, int(output_interval), fe3, int(max_intervals)))
+        self._hnemd = (int(output_interval), int(max_intervals))
+
+    def hnemd_take(self, temperature):
+        """(kappa[n, 5] in W/mK, rows[n, output_interval, 5]) of the n intervals finished since the last
+        take; an unfinished interval carries over."""
+        oi, mx = self._hnemd
+        kappa, rows, n = np.zeros(5 * mx), np.zeros(5 * oi * mx), C.c_int(0)
+        dp = C.POINTER(C.c_double)
+        _check(self._L.b200md_mgpu_hnemd_take(self._h, float(temperature), C.byref(n), kappa.ctypes.data_as(dp),
+                                              rows.ctypes.data_as(dp)))
+        m = n.value
+        return kappa[:5 * m].reshape(m, 5), rows[:5 * oi * m].reshape(m, oi, 5)
 
     def info(self, what, k=0):
         return int(self._L.b200md_mgpu_info(self._h, int(what), int(k)))

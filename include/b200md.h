@@ -319,6 +319,35 @@ int b200md_hnemd_sample(
 int b200md_hnemd_take(
   b200md_hnemd* p, double volume, double temperature, double* kappa5, double* rows, void* stream);
 
+/* The same drive, heat sums and kappa for a system held in several arrays (libb200md_mgpu's blocks),
+ * whose force total is combined by the caller and whose sampled step lives on the device:
+ *   b200md_hnemd_drive_add      f_i += W_i^T fe for i < n (the per-atom add of b200md_hnemd_drive) and
+ *                               the total of the new forces into d_ftot[3] (device); n = 0 is one
+ *                               thread block that writes a zero total.  d_scratch as for
+ *                               b200md_hnemd_drive (b200md_hnemd_drive_scratch_bytes(n), ticket zeroed)
+ *   b200md_hnemd_drive_correct  f_i -= d_ftot[.] * one_over_n for i < n (gpu_correct_force with the
+ *                               caller's 1.0 / N); n = 0 launches nothing.  b200md_hnemd_drive is
+ *                               _add then _correct with 1.0 / n.
+ *   b200md_hnemd_heat_row       the heat-current sum of atoms [0, n) (as b200md_hnemd_sample) into row
+ *                               *d_row of d_rows[n_rows][5]; the kernel then sets *d_row = (*d_row + 1)
+ *                               % n_rows on the device, so one captured launch serves every step.
+ *                               d_scratch: b200md_hnemd_heat_row_scratch_bytes(n) bytes, zeroed before
+ *                               the first call; n = 0 writes a zero row
+ *   b200md_hnemd_kappa          kappa5 of one interval from its host rows[output_interval * 5], the
+ *                               formula of b200md_hnemd_take */
+int b200md_hnemd_drive_add(
+  int n, int stride, const double fe[3], const double* d_virial, double* d_force, void* d_scratch,
+  double* d_ftot, void* stream);
+int b200md_hnemd_drive_correct(
+  int n, int stride, double one_over_n, const double* d_ftot, double* d_force, void* stream);
+long long b200md_hnemd_heat_row_scratch_bytes(int n);
+int b200md_hnemd_heat_row(
+  int n, int stride, const double* d_virial, const double* d_velocity, double* d_rows, int n_rows,
+  unsigned int* d_row, void* d_scratch, void* stream);
+int b200md_hnemd_kappa(
+  int output_interval, double volume, double temperature, const double fe[3], const double* rows,
+  double* kappa5);
+
 /* Spectral heat current (SHC), on the time-correlation engine of DOS, SDC and MSD (b2_correlate.cu,
  * below).  Replaces SHC::parse / preprocess / process / postprocess (src/measure/shc.cu:34-542):
  *   b200md_shc_create  <- parse (:466-542) + preprocess (:34-79).  Output groups: num_groups sizes and

@@ -73,6 +73,31 @@ int b200md_mgpu_thermo(b200md_mgpu* g, double out8[8]);
 /* global heat current jx_in, jx_out, jy_in, jy_out, jz (compute_heat.cu:32-90 summed, hac.cu:51,106) */
 int b200md_mgpu_heat_current(b200md_mgpu* g, double out5[5]);
 
+/* HNEMD thermal conductivity (Fan et al., PRB 99, 064308 (2019)) inside the step, which becomes
+ * VV1 -> halo -> potential -> drive -> VV2 -> thermostat -> heat row (Run::perform_a_run's order):
+ *   drive     compute_hnemd's branch of Force::compute, src/force/force.cu:857-897: every block adds
+ *             W_i^T fe to the forces of its owned atoms (the per-atom add of b200md_hnemd_drive, bit for
+ *             bit), the blocks' totals of the new forces are summed (a 3-double ncclAllReduce; local
+ *             mode: in block order) and every owned atom loses total / N;
+ *   heat row  HNEMD::process, src/measure/hnemd_kappa.cu:82-106: every block sums the heat current of
+ *             its owned atoms into a device row whose index lives on the device, so one captured graph
+ *             serves every step; the blocks' rows are summed only by b200md_mgpu_hnemd_take.
+ * b200md_mgpu_hnemd_set: call after b200md_mgpu_distribute (which switches HNEMD off).  fe[3] in 1/A;
+ *   fe = 0 switches HNEMD off (Force::finalize).  Re-evaluates the forces at the current positions,
+ *   driven when HNEMD is on, as the reference does before a run's loop (run.cu:217-248), discards the
+ *   captured step and starts a new series.  Refuses output_interval < 1, max_intervals < 1 and a
+ *   non-finite fe.  A b200md_mgpu_run that would leave more than max_intervals whole intervals untaken
+ *   returns B200MD_ERR_OVERFLOW before it launches anything.
+ * b200md_mgpu_hnemd_take: the output branch of HNEMD::process, hnemd_kappa.cu:108-131 (synchronises;
+ *   the only HNEMD call that does).  *n_intervals = the intervals completed since the last take; for
+ *   each, in order, kappa[5 j + k] (W/mK, k = xx_in xx_out yy_in yy_out zz; the factor of
+ *   b200md_hnemd_take with the volume Lx Ly Lz) and, if rows != NULL, its output_interval global heat
+ *   sums rows[(j * output_interval + m) * 5 + k].  kappa holds 5 * max_intervals doubles, rows
+ *   5 * output_interval * max_intervals.  The steps of an unfinished interval carry over. */
+int b200md_mgpu_hnemd_set(b200md_mgpu* g, int output_interval, const double fe[3], int max_intervals);
+int b200md_mgpu_hnemd_take(
+  b200md_mgpu* g, double temperature, int* n_intervals, double* kappa, double* rows);
+
 /* counters: what = 0 local domains, 1 owned atoms of domain k, 2 local (owned+ghost) atoms of
  * domain k, 3 migrations so far, 4 neighbour rebuilds of domain k, 5 global rank of domain k,
  * 6 kernels launched per step (this module's + libb200md's, counted on the last eager step) */
