@@ -570,6 +570,7 @@ emu_lj* emu_lj_create(int nt, const double* para, int n)
   return p;
 }
 void emu_lj_destroy(emu_lj* p) { delete p; }
+int emu_lj_error_bits(emu_lj* p) { return p->nb.flags[1]; }
 int emu_lj_compute(
   emu_lj* p, int n, const double h[9], const int pbc[3], const int* type, const double* pos,
   double* pe, double* force, double* virial)
@@ -648,6 +649,7 @@ emu_tersoff* emu_tersoff_create(int nt, const double* para, int n)
   return p;
 }
 void emu_tersoff_destroy(emu_tersoff* p) { delete p; }
+int emu_tersoff_error_bits(emu_tersoff* p) { return p->nb.flags[1]; }
 int emu_tersoff_compute(
   emu_tersoff* p, int n, const double h[9], const int pbc[3], const int* type, const double* pos,
   double* pe, double* force, double* virial)
@@ -730,6 +732,7 @@ emu_eam* emu_eam_create(int model, int nt, const double* para, int n)
   return p;
 }
 void emu_eam_destroy(emu_eam* p) { delete p; }
+int emu_eam_error_bits(emu_eam* p) { return p->nb.flags[1]; }
 int emu_eam_compute(
   emu_eam* p, int n, const double h[9], const int pbc[3], const int* type, const double* pos,
   double* pe, double* force, double* virial)

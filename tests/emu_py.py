@@ -146,6 +146,8 @@ class Emu:
         E.emu_nep_create.argtypes = [C.c_char_p, C.c_int]
         E.emu_nep_destroy.argtypes = [C.c_void_p]
         E.emu_nep_rebuilds.argtypes = [C.c_void_p]
+        for k in ("nep", "lj", "tersoff", "eam"):
+            getattr(E, f"emu_{k}_error_bits").argtypes = [C.c_void_p]
         E.emu_nep_compute.argtypes = [C.c_void_p, C.c_int, _dp, _ip, _ip, _dp, _dp, _dp, _dp]
         E.emu_nep_export_neighbors.argtypes = [C.c_void_p, C.c_int, _ip, _ip, C.c_int, _ip, _ip]
         E.emu_nep_export_skin.argtypes = [C.c_void_p, C.c_int, _ip, _ip]
