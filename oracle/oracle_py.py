@@ -474,10 +474,12 @@ def baoab_operator(which, dt, mass, pos, vel, force, label=None, fixed_group=-1)
     return p, v
 
 
-def berendsen_pressure(h, pbc, thermo, target_p, p_coupling, num_components):
-    """cpu_pressure_isotropic / _orthogonal / _triclinic, src/integrate/ensemble_ber.cu:88-172 (no
-    deformation): returns (new h[9], mu[9]); positions transform as r <- mu r.  thermo[2..7] = sxx syy szz
-    sxy sxz syz; target_p / p_coupling in natural units, Voigt order xx yy zz yz xz xy for 6 components."""
+def berendsen_pressure(h, pbc, thermo, target_p, p_coupling, num_components, deform=None, deform_rate=None):
+    """cpu_pressure_isotropic / _orthogonal / _triclinic, src/integrate/ensemble_ber.cu:88-172: returns
+    (new h[9], mu[9]); positions transform as r <- mu r.  thermo[2..7] = sxx syy szz sxy sxz syz; target_p /
+    p_coupling in natural units, Voigt order xx yy zz yz xz xy for 6 components.  deform[3] / deform_rate[3]
+    (3 components only, `deform`): a deformed direction grows by its rate (A per step) whether it is
+    periodic or open, s = (h + rate) / h; that test comes before the pbc test."""
     h = np.array(h, dtype=np.float64).reshape(9)
     p = np.asarray(thermo, dtype=np.float64)[2:8]
     p0, pc = np.asarray(target_p, dtype=np.float64), np.asarray(p_coupling, dtype=np.float64)
@@ -488,7 +490,10 @@ def berendsen_pressure(h, pbc, thermo, target_p, p_coupling, num_components):
         h[[0, 4, 8]] *= sfac
     elif num_components == 3:
         for d in range(3):
-            sfac = 1.0 - pc[d] * (p0[d] - p[d]) if pbc[d] else 1.0
+            if deform is not None and deform[d]:
+                sfac = (h[4 * d] + deform_rate[d]) / h[4 * d]
+            else:
+                sfac = 1.0 - pc[d] * (p0[d] - p[d]) if pbc[d] else 1.0
             mu[4 * d] = sfac
             h[4 * d] *= sfac
     else:

@@ -132,6 +132,24 @@ def test_open_direction_and_stiff_direction_keep_their_box(kind):
     assert (h[0] != s["h"][0]) == (kind == "npt_ber")
 
 
+@pytest.mark.parametrize("pbc", [(1, 1, 1), (1, 1, 0)])
+def test_deform_overrides_the_pressure_and_the_open_direction(oracle, pbc):
+    """`deform` in the 3-component barostat: the deformed directions grow by their rate per step, open or
+    not; the others keep the pressure rule (periodic) or their length (open)."""
+    h = np.diag([40.0, 41.0, 42.0]).reshape(9)
+    thermo = np.array([300.0, -1.0, 0.010, 0.012, 0.008, 0.0, 0.0, 0.0])
+    p0, pc = np.array([0.003, 0.002, 0.001]), np.array([0.5, 0.4, 0.3])
+    plain, mu0 = oracle.berendsen_pressure(h, pbc, thermo, p0, pc, 3)
+    hn, mu = oracle.berendsen_pressure(h, pbc, thermo, p0, pc, 3, deform=(1, 0, 1), deform_rate=(1e-3, 5.0, -2e-3))
+    assert hn[0] == pytest.approx(40.001, rel=1e-15) and hn[8] == pytest.approx(41.998, rel=1e-15)
+    assert mu[0] == hn[0] / 40.0 and mu[8] == hn[8] / 42.0
+    assert hn[4] == plain[4] and mu[4] == mu0[4]  # y is not deformed: its rate is not read
+    assert hn[4] != 41.0
+    assert np.array_equal(hn[[1, 2, 3, 5, 6, 7]], np.zeros(6))
+    assert np.array_equal(oracle.berendsen_pressure(h, pbc, thermo, p0, pc, 3, deform=(0, 0, 0),
+                                                    deform_rate=(1.0, 1.0, 1.0))[0], plain)
+
+
 def harmonic_run(dt, steps, k_spring=2.0, n=64, seed=7):
     """NVE on independent 3D oscillators f = -k (r - r0); returns the total energy after every step."""
     rng = np.random.default_rng(seed)
