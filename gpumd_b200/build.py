@@ -19,7 +19,7 @@ OBJ = PKG / "build"
 
 CU_SOURCES = ["b2_host.cu", "b2_neighbor.cu", "b2_nep.cu", "b2_md.cu", "b2_tersoff.cu", "b2_eam.cu",
               "b2_tc_test.cu", "b2_stochastic.cu", "b2_measure.cu", "b2_nemd.cu", "b2_correlate.cu",
-              "b2_minimize.cu", "b2_phonon.cu"]
+              "b2_minimize.cu", "b2_phonon.cu", "b2_rdf.cu"]
 CPP_SOURCES = ["b2_nep_model.cpp"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -493,6 +493,57 @@ int Neighbor::update(
   return B200MD_OK;
 }
 
+int Neighbor::sort_cells(
+  const B2Box& box, const int* d_type, const double* d_pos, int n_in, double cell_size, cudaStream_t st)
+{
+  if (n_in <= 0 || n_in > capacity) {
+    set_error("sort_cells: the number of atoms must be in 1 .. the capacity given at construction");
+    return B200MD_ERR_ARG;
+  }
+  if (n_in != n) {
+    const int rc_inv = invalidate(n_in, st);
+    if (rc_inv != B200MD_OK)
+      return rc_inv;
+  }
+  const B2Grid g = make_grid(box, cell_size);
+  for (int d = 0; d < 3; ++d) {
+    if (box.pbc[d] && g.nb[d] < 5) {
+      set_error("sort_cells: fewer than 5 cells in a periodic direction (box thinner than 2.5 cutoffs)");
+      return B200MD_ERR_SMALL_BOX;
+    }
+  }
+  if ((size_t)g.ncell + 1 > cell_start.n) {
+    const size_t cap = (size_t)(g.ncell * 1.2) + 64;
+    B2_CUDA(cudaStreamSynchronize(st));
+    B2_CUDA(cell_count.reserve(cap));
+    B2_CUDA(cell_fill.reserve(cap));
+    B2_CUDA(cell_start.reserve(cap + 1));
+  }
+  grid = g;
+  have_grid = true;
+  const B2NeighborView v = view();
+  const int gn = grid_for(n, BLK), gc = grid_for(g.ncell, BLK);
+  k_force_rebuild<<<1, 1, 0, st>>>(flags.p);
+  B2_LAUNCHED();
+  k_pack_check<<<gn, BLK, 0, st>>>(v, box, d_type, d_pos, d_pos + n, d_pos + 2 * (size_t)n, 0.0f);
+  B2_LAUNCHED();
+  k_zero_cells<<<gc, BLK, 0, st>>>(v, g.ncell);
+  B2_LAUNCHED();
+  k_cell_count<<<gn, BLK, 0, st>>>(v, box, g);
+  B2_LAUNCHED();
+  k_scan_cells<<<1, 1024, 0, st>>>(v, g.ncell);
+  B2_LAUNCHED();
+  k_cell_fill<<<gn, BLK, 0, st>>>(v);
+  B2_LAUNCHED();
+  k_sort_cells<<<gc, BLK, 0, st>>>(v, g.ncell);
+  B2_LAUNCHED();
+  k_commit<<<gn, BLK, 0, st>>>(v);
+  B2_LAUNCHED();
+  k_rebuild_done<<<1, 1, 0, st>>>(flags.p);
+  B2_LAUNCHED();
+  return B200MD_OK;
+}
+
 int Neighbor::enable_schedule()
 {
   B2_CUDA(seg_order.reserve(((size_t)capacity + 31) / 32));

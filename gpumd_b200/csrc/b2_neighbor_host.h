@@ -58,6 +58,11 @@ public:
   // Neighbor::find_neighbor_global, src/force/neighbor.cu:756-800 (fully asynchronous here)
   int update(const B2Box& box, const int* d_type, const double* d_pos, int n, cudaStream_t st);
   int check(cudaStream_t st, int* err_bits, int* rebuilds);
+  // cells only, for consumers with their own pair loop (the RDF): re-sort the atoms by cells of at least
+  // cell_size, every call, and build no skin list (init with mn_skin = 0).  atoms / cell_start / perm of
+  // view() then hold the sorted records of d_pos; update() is not to be mixed with it on one object
+  int sort_cells(const B2Box& box, const int* d_type, const double* d_pos, int n, double cell_size,
+                 cudaStream_t st);
   // forget the current ordering and lists (the caller changed the atom set or its order)
   int invalidate(int n_new, cudaStream_t st);
   B2NeighborView view() const;

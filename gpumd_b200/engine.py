@@ -414,6 +414,51 @@ class HAC:
         return hac.reshape(5, self.Nc), rtc.reshape(5, self.Nc)
 
 
+class RDF:
+    """compute_rdf, src/measure/rdf.cu:128-333: total and partial radial distribution functions.
+    The species are the types present in type_ (host array), in type-id order.  process(box, atom)
+    takes one sample (the caller picks the steps, (step + 1) % interval == 0 in the reference);
+    postprocess(num_repeats) returns [num_bins, 1 + T (T + 1) / 2]: total, then (a, b) for a <= b."""
+
+    def __init__(self, rc, num_bins, type_):
+        _require_cuda()
+        self._L = _lib.load()
+        t = np.asarray(type_, dtype=np.int64).reshape(-1)
+        counts = np.bincount(t, minlength=1) if t.size else np.zeros(1, np.int64)
+        self.type_index = np.ascontiguousarray(np.nonzero(counts)[0], dtype=np.int32)
+        self.num_atoms = np.ascontiguousarray(counts[self.type_index], dtype=np.int32)
+        self.n, self.rc, self.num_bins = int(t.size), float(rc), int(num_bins)
+        self.num_types = int(self.type_index.size)
+        self.num_RDFs = 1 + self.num_types * (self.num_types + 1) // 2
+        self.dr = self.rc / self.num_bins
+        ip = C.POINTER(C.c_int)
+        h = C.c_void_p()
+        _lib.check(self._L.b200md_rdf_create(self.rc, self.num_bins, self.num_types,
+                                             self.type_index.ctypes.data_as(ip), self.num_atoms.ctypes.data_as(ip),
+                                             self.n, C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.b200md_rdf_destroy(self._h)
+            self._h = None
+
+    @property
+    def radius(self):
+        """r_mid of every bin as rdf.out prints it (bin * dr + dr / 2, rdf.cu:238)"""
+        return np.arange(self.num_bins) * self.dr + self.dr / 2
+
+    def process(self, box, atom):
+        _lib.check(self._L.b200md_rdf_sample(self._h, box._h, box._p, _ptr(atom.type),
+                                             _ptr(atom.position_per_atom), self.n, _stream()))
+
+    def postprocess(self, num_repeats):
+        out = np.zeros(self.num_bins * self.num_RDFs)
+        _lib.check(self._L.b200md_rdf_finish(self._h, int(num_repeats), out.ctypes.data_as(C.POINTER(C.c_double)),
+                                             _stream()))
+        return out.reshape(self.num_bins, self.num_RDFs)
+
+
 class Force:
     """Force driver, src/force/force.cu: parse_potential (75-218) and compute (771-985)."""
 

@@ -664,6 +664,135 @@ private:
   b200md_msd* msd_ = nullptr;
 };
 
+// compute_rdf rc num_bins interval (RDF::parse, rdf.cu:264-333).  The species are the types with at least
+// one atom, in type-id order.  One deliberate difference: a run shorter than one interval is refused,
+// where the reference divides by num_repeats = 0
+class ComputeRdf : public Property
+{
+public:
+  ComputeRdf(const MeasureContext& ctx, const std::vector<std::string>& t)
+  {
+    printf("Compute radial distribution function (RDF).\n");
+    if (t.size() != 4)
+      input_error("compute_rdf should have 3 parameters.");
+    if (!valid_real(t[1], &rc_))
+      input_error("radial cutoff should be a number.");
+    if (rc_ <= 0)
+      input_error("radial cutoff should be positive.");
+    const Box& box = ctx.model.box;
+    const double volume = box.get_volume();
+    for (int d = 0; d < 3; ++d) { // every direction, open ones included (rdf.cu:283-292)
+      if (rc_ > volume / area(box, d) / 2.5)
+        input_error("The box has a thickness < 2.5 RDF radial cutoffs in a periodic direction.\n"
+                    "                Please increase the periodic direction(s).");
+    }
+    printf("    radial cutoff %g.\n", rc_);
+    if (!valid_int(t[2], &num_bins_))
+      input_error("number of bins should be an integer.");
+    if (num_bins_ <= 20)
+      input_error("A larger nbins is recommended.");
+    if (num_bins_ > 500)
+      input_error("A smaller nbins is recommended.");
+    printf("    radial cutoff will be divided into %d bins.\n", num_bins_);
+    if (!valid_int(t[3], &interval_))
+      input_error("interval step per sample should be an integer.");
+    if (interval_ <= 0)
+      input_error("interval step per sample should be positive.");
+    printf("    RDF sample interval is %d step.\n", interval_);
+    const Atom& a = ctx.model.atom;
+    std::vector<int> size;
+    for (int n = 0; n < a.number_of_atoms; ++n) {
+      if (a.cpu_type[n] >= (int)size.size())
+        size.resize(a.cpu_type[n] + 1, 0);
+      ++size[a.cpu_type[n]];
+    }
+    for (int ty = 0; ty < (int)size.size(); ++ty) {
+      if (size[ty] != 0) {
+        type_index_.push_back(ty);
+        num_atoms_.push_back(size[ty]);
+      }
+    }
+    const int T = (int)type_index_.size();
+    printf("    There are %d atom types in model.xyz.\n", T);
+    for (int k = 0; k < T; ++k)
+      printf("        Type %d has %d atoms.\n", type_index_[k], num_atoms_[k]);
+    printf("    Will calculate one total RDF and %d partial RDFs.\n", T * (T + 1) / 2);
+  }
+  ~ComputeRdf() override { b200md_rdf_destroy(rdf_); }
+  void preprocess(const MeasureContext& ctx, int number_of_steps) override // rdf.cu:163-176
+  {
+    num_repeats_ = number_of_steps / interval_;
+    if (num_repeats_ < 1)
+      input_error("compute_rdf: the run has fewer steps than one sample interval.");
+    b200md_rdf_destroy(rdf_);
+    rdf_ = nullptr;
+    check_create("compute_rdf", b200md_rdf_create(rc_, num_bins_, (int)type_index_.size(), type_index_.data(),
+                                                  num_atoms_.data(), ctx.model.atom.number_of_atoms, &rdf_));
+  }
+  void process(const MeasureContext& ctx, int step) override // rdf.cu:178-202
+  {
+    if ((step + 1) % interval_ != 0)
+      return;
+    const Box& box = ctx.model.box;
+    int pbc[3];
+    box.pbc(pbc);
+    const Atom& a = ctx.model.atom;
+    if (b200md_rdf_sample(rdf_, box.cpu_h, pbc, a.type.data(), a.position_per_atom.data(), a.number_of_atoms,
+                          nullptr) != B200MD_OK)
+      b2h_fail("compute_rdf");
+  }
+  // RDF::postprocess, rdf.cu:204-251: appended to rdf.out
+  void postprocess(const MeasureContext& ctx) override
+  {
+    const int T = (int)type_index_.size(), R = 1 + T * (T + 1) / 2;
+    std::vector<double> g((size_t)num_bins_ * R);
+    if (b200md_rdf_finish(rdf_, num_repeats_, g.data(), nullptr) != B200MD_OK)
+      b2h_fail("compute_rdf");
+    const Atom& a = ctx.model.atom;
+    std::vector<std::string> symbol(T);
+    for (int k = 0; k < T; ++k) {
+      for (int n = 0; n < a.number_of_atoms; ++n) {
+        if (a.cpu_type[n] == type_index_[k]) {
+          symbol[k] = a.cpu_atom_symbol[n];
+          break;
+        }
+      }
+    }
+    FILE* fid = open_output("rdf.out", "a");
+    fprintf(fid, "#radius total");
+    for (int p = 0; p < T; p++)
+      for (int q = p; q < T; q++)
+        fprintf(fid, " %s-%s", symbol[p].c_str(), symbol[q].c_str());
+    fprintf(fid, "\n");
+    const double dr = rc_ / num_bins_;
+    for (int bin = 0; bin < num_bins_; bin++) {
+      fprintf(fid, "%.5f", bin * dr + dr / 2);
+      for (int k = 0; k < R; ++k)
+        fprintf(fid, " %.5f", g[(size_t)bin * R + k]);
+      fprintf(fid, "\n");
+    }
+    fclose(fid);
+  }
+
+private:
+  // Box::get_area, box.cu:34-48
+  static double area(const Box& box, int d)
+  {
+    const double* h = box.cpu_h;
+    const double col[3][3] = {{h[0], h[3], h[6]}, {h[1], h[4], h[7]}, {h[2], h[5], h[8]}};
+    const double* u = col[(d + 1) % 3];
+    const double* w = col[(d + 2) % 3];
+    const double s1 = u[1] * w[2] - u[2] * w[1];
+    const double s2 = u[2] * w[0] - u[0] * w[2];
+    const double s3 = u[0] * w[1] - u[1] * w[0];
+    return sqrt(s1 * s1 + s2 * s2 + s3 * s3);
+  }
+  double rc_ = 0.0;
+  int num_bins_ = 0, interval_ = 0, num_repeats_ = 0;
+  std::vector<int> type_index_, num_atoms_;
+  b200md_rdf* rdf_ = nullptr;
+};
+
 // dump_thermo interval: T, K, U, then sxx syy szz syz sxz sxy in GPa, then the box (dump_thermo.cu:73-129)
 class DumpThermo : public Property
 {
@@ -893,8 +1022,8 @@ const struct {
 } KEYWORDS[] = {
   {"compute_hac", make<ComputeHac>},   {"compute_hnemd", make<ComputeHnemd>}, {"compute", make<Compute>},
   {"compute_shc", make<ComputeShc>},   {"compute_dos", make<ComputeDos>},     {"compute_sdc", make<ComputeSdc>},
-  {"compute_msd", make<ComputeMsd>},   {"dump_thermo", make<DumpThermo>},     {"dump_xyz", make<DumpXyz>},
-  {"dump_restart", make<DumpRestart>},
+  {"compute_msd", make<ComputeMsd>},   {"compute_rdf", make<ComputeRdf>},     {"dump_thermo", make<DumpThermo>},
+  {"dump_xyz", make<DumpXyz>},         {"dump_restart", make<DumpRestart>},
 };
 const size_t NUM_KEYWORDS = sizeof(KEYWORDS) / sizeof(KEYWORDS[0]);
 

@@ -111,6 +111,10 @@ SIGNATURES = {
     "b200md_msd_destroy": (None, [_vp]),
     "b200md_msd_sample": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp]),
     "b200md_msd_finish": (C.c_int, [_vp, _dp, _dp, _vp]),
+    "b200md_rdf_create": (C.c_int, [C.c_double, C.c_int, C.c_int, _ip, _ip, C.c_int, C.POINTER(_vp)]),
+    "b200md_rdf_destroy": (None, [_vp]),
+    "b200md_rdf_sample": (C.c_int, [_vp, _dp, _ip, _vp, _vp, C.c_int, _vp]),
+    "b200md_rdf_finish": (C.c_int, [_vp, C.c_int, _dp, _vp]),
     "b200md_unwrap_begin": (C.c_int, [C.c_int, _vp, _vp, _vp]),
     "b200md_unwrap_end": (C.c_int, [C.c_int, _vp, _vp, _vp, _vp]),
     "b200md_heat_bath_create":(C.c_int, [C.c_int, C.c_int, C.c_int, _ip, _ip, C.c_int, C.c_int, C.c_double,

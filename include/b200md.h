@@ -434,6 +434,29 @@ int b200md_unwrap_begin(int n, const double* d_position, double* d_position_old,
 int b200md_unwrap_end(
   int n, const double* d_position, const double* d_position_old, double* d_unwrapped, void* stream);
 
+/* Radial distribution function (b2_rdf.cu).  Replaces RDF::parse / preprocess / process / postprocess
+ * (src/measure/rdf.cu:128-333, rdf.cuh:27-41):
+ *   b200md_rdf_create   <- parse (:264-333) + preprocess (:163-176).  num_types species, the types with at
+ *                          least one atom in ascending type id (type_index[], < 94), with num_atoms[] atoms
+ *                          each, n atoms in all (the sum).  dr = rc / num_bins.  B200MD_ERR_ARG, with the
+ *                          reference's message, for rc <= 0, num_bins <= 20 or > 500.  The box-thickness
+ *                          check (:283-292) needs the box: a sample in a box with fewer than 5 cells of rc / 2
+ *                          in a periodic direction returns B200MD_ERR_SMALL_BOX.
+ *   b200md_rdf_sample   <- process (:178-202) + find_rdf (:128-161): one sample at these positions, with the
+ *                          volume of box_h[9] (row-major, lattice vectors as columns); d_pos [3][n] SoA.  Each
+ *                          unordered pair within rc is counted once into 64-bit integer bins and the sample
+ *                          is folded into the FP64 accumulator on the device.  Asynchronous.
+ *   b200md_rdf_finish   <- postprocess (:204-251): out[num_bins][1 + num_types (num_types + 1) / 2] = the
+ *                          accumulated total and partial (a, b), a <= b, RDFs divided by num_repeats
+ *                          (number_of_steps / interval; must be >= 1).  Synchronises; the only copy. */
+typedef struct b200md_rdf b200md_rdf;
+int b200md_rdf_create(
+  double rc, int num_bins, int num_types, const int* type_index, const int* num_atoms, int n, b200md_rdf** out);
+void b200md_rdf_destroy(b200md_rdf* p);
+int b200md_rdf_sample(
+  b200md_rdf* p, const double* box_h, const int* pbc, const int* d_type, const double* d_pos, int n, void* stream);
+int b200md_rdf_finish(b200md_rdf* p, int num_repeats, double* out, void* stream);
+
 /* Direct NEMD: heat source / sink baths and group averages.
  *   b200md_heat_bath_create  <- the heat branches of the Ensemble_LAN / _NHC / _BDP constructors
  *                               (ensemble_lan.cu:43-85, ensemble_nhc.cu:52-91, ensemble_bdp.cu:50-62).

@@ -423,6 +423,24 @@ def main():
                     model_file=GOLDEN / "ref_silicon_liquid_restart1.xyz")
     infos.append(i)
 
+    # radial distribution functions (rdf.out): one static sample of each case of tests/test_gpu_rdf.py at 21
+    # and 500 bins, and a 200-step PbTe NVE run sampled every 20 steps -> refgpu_rdf_<case>_<bins>.out.gz,
+    # refgpu_rdf_pbte_nve.out.gz
+    import gzip
+    import rdf_support
+    for case, (s, rc, sym, pot) in rdf_support.rdf_cases().items():
+        for nb in rdf_support.RDF_BINS:
+            d, i = run_case(f"rdf_{case}_{nb}", s, sym, pot, rdf_support.RDF_STATIC.format(rc=rc, nb=nb))
+            if d is not None:
+                (OUT / f"refgpu_rdf_{case}_{nb}.out.gz").write_bytes(gzip.compress((d / "rdf.out").read_bytes(),
+                                                                                   mtime=0))
+            infos.append(i)
+    s, vel, sym, pot = rdf_support.rdf_nve_case()
+    d, i = run_case("rdf_pbte_nve", s, sym, pot, rdf_support.RDF_NVE_RUN, vel)
+    if d is not None:
+        (OUT / "refgpu_rdf_pbte_nve.out.gz").write_bytes(gzip.compress((d / "rdf.out").read_bytes(), mtime=0))
+    infos.append(i)
+
     # ---- (3) throughput at the BASELINE sizes ----
     if not args.skip_speed:
         s = rocksalt_pbte(50, rattle=0.02, seed=1)  # C3: 1 000 000 atoms
