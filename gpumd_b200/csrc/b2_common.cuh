@@ -11,6 +11,7 @@
 
 #if defined(__CUDACC__)
 #define B2_HD __device__ __forceinline__
+#define B2_HOST_DEVICE __host__ __device__ // sizes both the kernels and the host setup (b2_setup.h) compute
 #define B2_LDG(p) __ldg(p)
 // streaming (evict-first) load / store for data that is touched once per kernel -- the neighbour
 // lists -- so that it does not displace the gathered records and U rows from L1 / L2
@@ -18,6 +19,7 @@
 #define B2_STCS(p, v) __stcs((p), (v))
 #else
 #define B2_HD static inline
+#define B2_HOST_DEVICE
 #define B2_LDG(p) (*(p))
 #define B2_LDCS(p) (*(p))
 #define B2_STCS(p, v) (*(p) = (v))

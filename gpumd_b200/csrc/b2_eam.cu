@@ -72,129 +72,35 @@ int b200md_eam_create(const char* path, int num_atoms, b200md_eam** out)
     set_error("b200md_eam_create: no CUDA device (libb200md has no CPU fallback)");
     return B200MD_ERR_CUDA;
   }
-  FILE* fid = fopen(path, "r");
-  if (!fid) {
-    set_error(std::string("Failed to open ") + path);
-    return B200MD_ERR_IO;
-  }
-  char name[64];
-  int nt = 0;
-  if (fscanf(fid, "%63s%d", name, &nt) != 2) {
-    fclose(fid);
-    set_error("Reading error for EAM potential.");
-    return B200MD_ERR_ARG;
-  }
-  int model = -1;
-  if (std::strcmp(name, "eam_zhou_2004") == 0)
-    model = 0;
-  else if (std::strcmp(name, "eam_dai_2006") == 0)
-    model = 1;
-  if (model < 0 || nt < 1 || nt > 18 || (model == 1 && nt != 1)) {
-    fclose(fid);
-    set_error("EAM potential file: expected 'eam_zhou_2004 <1..18> ...' or 'eam_dai_2006 1 ...'");
-    return B200MD_ERR_ARG;
-  }
+  EamFile file;
+  const std::string err = load_eam(path, file);
+  if (!err.empty())
+    return load_error(err);
   b200md_eam* p = new (std::nothrow) b200md_eam;
   if (!p) {
-    fclose(fid);
     set_error("out of host memory");
     return B200MD_ERR_ARG;
   }
-  p->nt = nt;
-  p->model = model;
-  for (int k = 0; k < nt; ++k) {
-    if (fscanf(fid, "%63s", name) != 1) {
-      fclose(fid);
-      delete p;
-      set_error("Reading error for EAM potential.");
-      return B200MD_ERR_ARG;
-    }
-    p->symbols.push_back(name);
-  }
-  B2EamView& P = p->view;
-  std::memset(&P, 0, sizeof P);
-  std::vector<float> zp((size_t)nt * EZ_COUNT, 0.0f);
-  float rc = 0.0f;
-  bool ok = true;
-  if (model == 0) { // eam.cu:46-92
-    for (int t = 0; t < nt && ok; ++t) {
-      float x[21];
-      for (int k = 0; k < 21; ++k)
-        ok = ok && fscanf(fid, "%f", &x[k]) == 1;
-      float* e = &zp[(size_t)t * EZ_COUNT];
-      e[EZ_RE_INV] = 1.0f / x[0];
-      e[EZ_FE] = x[1];
-      e[EZ_RHO_E_INV] = 1.0f / x[2];
-      e[EZ_RHO_S_INV] = 1.0f / x[3];
-      e[EZ_ALPHA] = x[4];
-      e[EZ_BETA] = x[5];
-      e[EZ_A] = x[6];
-      e[EZ_B] = x[7];
-      e[EZ_KAPPA] = x[8];
-      e[EZ_LAMBDA] = x[9];
-      e[EZ_FN0] = x[10];
-      e[EZ_FN1] = x[11];
-      e[EZ_FN2] = x[12];
-      e[EZ_FN3] = x[13];
-      e[EZ_F0] = x[14];
-      e[EZ_F1] = x[15];
-      e[EZ_F2] = x[16];
-      e[EZ_F3] = x[17];
-      e[EZ_ETA] = x[18];
-      e[EZ_FE_EMBED] = x[19];
-      e[EZ_RC] = x[20];
-      e[EZ_RHO_N] = x[2] * 0.85;
-      e[EZ_RHO_0] = x[2] * 1.15;
-      e[EZ_RHO_N_INV] = 1.0f / e[EZ_RHO_N];
-      if (rc < x[20])
-        rc = x[20];
-    }
-  } else { // eam.cu:94-122
-    float x[9];
-    for (int k = 0; k < 9; ++k)
-      ok = ok && fscanf(fid, "%f", &x[k]) == 1;
-    P.dA = x[0];
-    P.dd = x[1];
-    P.dc = x[2];
-    P.dc0 = x[3];
-    P.dc1 = x[4];
-    P.dc2 = x[5];
-    P.dc3 = x[6];
-    P.dc4 = x[7];
-    P.dB = x[8];
-    rc = P.dc > P.dd ? P.dc : P.dd;
-  }
-  fclose(fid);
-  if (!ok) {
-    delete p;
-    set_error("Reading error for EAM potential.");
-    return B200MD_ERR_ARG;
-  }
-  p->rc = rc;
+  p->nt = file.nt;
+  p->model = file.view.model;
+  p->symbols = file.symbols;
+  p->rc = file.rc;
   p->n = num_atoms;
   const size_t N = (size_t)num_atoms;
-  // neighbor.initialize(rc, number_of_atoms, 400), eam.cu:43 ("very safe for EAM"); bounded here by
-  // what a sphere of rc+skin can hold at twice fcc-metal density
-  const double rs = rc + 1.0;
-  int mn = (int)(400 * rs * rs * rs / ((double)rc * rc * rc));
-  const int mn_dense = (int)(4.19 * rs * rs * rs * 0.2) + 32;
-  if (b2_tight_lists() && mn > mn_dense)
-    mn = mn_dense;
-  int r = p->nb.init(num_atoms, rc, mn);
+  int r = p->nb.init(num_atoms, file.rc, file.mn_skin);
   if (r != B200MD_OK) {
     delete p;
     return r;
   }
-  if (p->zp.reserve(zp.size()) != cudaSuccess || p->Fp.reserve(N) != cudaSuccess ||
+  if (p->zp.reserve(file.zp.size()) != cudaSuccess || p->Fp.reserve(N) != cudaSuccess ||
       p->acc.reserve(13 * N) != cudaSuccess) {
     delete p;
     set_error("out of device memory");
     return B200MD_ERR_CUDA;
   }
-  cudaMemcpy(p->zp.p, zp.data(), sizeof(float) * zp.size(), cudaMemcpyHostToDevice);
-  P.model = model;
-  P.nt = nt;
-  P.rc = rc;
+  cudaMemcpy(p->zp.p, file.zp.data(), sizeof(float) * file.zp.size(), cudaMemcpyHostToDevice);
+  B2EamView& P = p->view;
+  P = file.view;
   P.zp = p->zp.p;
   P.n = num_atoms;
   P.atoms = p->nb.atoms.p;

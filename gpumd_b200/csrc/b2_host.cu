@@ -1,7 +1,6 @@
-// b2_host.cu -- error string, launch counter, box helper.
+// b2_host.cu -- error string, launch counter, stage profiler.
 #include "../../include/b200md.h"
 #include "b2_host.h"
-#include <cmath>
 #include <cstdio>
 
 namespace b2 {
@@ -21,40 +20,10 @@ bool cuda_ok(cudaError_t e, const char* what, const char* file, int line)
   return false;
 }
 
-B2Box make_box(const double h[9], const int pbc[3])
+int load_error(const std::string& err)
 {
-  B2Box b;
-  double* c = b.h;
-  for (int d = 0; d < 9; ++d)
-    c[d] = h[d];
-  for (int d = 0; d < 3; ++d)
-    b.pbc[d] = pbc[d] ? 1 : 0;
-  // adjugate / determinant
-  c[9] = c[4] * c[8] - c[5] * c[7];
-  c[10] = c[2] * c[7] - c[1] * c[8];
-  c[11] = c[1] * c[5] - c[2] * c[4];
-  c[12] = c[5] * c[6] - c[3] * c[8];
-  c[13] = c[0] * c[8] - c[2] * c[6];
-  c[14] = c[2] * c[3] - c[0] * c[5];
-  c[15] = c[3] * c[7] - c[4] * c[6];
-  c[16] = c[1] * c[6] - c[0] * c[7];
-  c[17] = c[0] * c[4] - c[1] * c[3];
-  const double det = c[0] * c[9] + c[1] * c[12] + c[2] * c[15];
-  for (int d = 9; d < 18; ++d)
-    c[d] /= det;
-  b.volume = std::fabs(det);
-  for (int d = 0; d < 3; ++d) {
-    // area of the face spanned by the other two lattice vectors (columns of h)
-    const int p = (d + 1) % 3, q = (d + 2) % 3;
-    const double u[3] = {c[p], c[p + 3], c[p + 6]}, w[3] = {c[q], c[q + 3], c[q + 6]};
-    const double s0 = u[1] * w[2] - u[2] * w[1], s1 = u[2] * w[0] - u[0] * w[2],
-                 s2 = u[0] * w[1] - u[1] * w[0];
-    b.thickness[d] = b.volume / std::sqrt(s0 * s0 + s1 * s1 + s2 * s2);
-  }
-  b.ortho = c[1] == 0 && c[2] == 0 && c[3] == 0 && c[5] == 0 && c[6] == 0 && c[7] == 0;
-  for (int d = 0; d < 18; ++d)
-    b.hf[d] = (float)c[d];
-  return b;
+  g_error = err;
+  return err.rfind("Failed to open", 0) == 0 ? B200MD_ERR_IO : B200MD_ERR_ARG;
 }
 
 StageProfiler::~StageProfiler()

@@ -26,8 +26,9 @@ bool cuda_ok(cudaError_t e, const char* what, const char* file, int line);
     B2_CUDA(cudaPeekAtLastError());     \
   } while (0)
 
-// Box::get_inverse / get_volume / thickness / set_is_orthogonal (src/model/box.cu:26-117)
-B2Box make_box(const double h[9], const int pbc[3]);
+// records the message of a failed load (b2_setup.h, NepModel::load) and returns its code: B200MD_ERR_IO when
+// the file could not be opened, else B200MD_ERR_ARG
+int load_error(const std::string& err);
 
 template <typename T>
 struct DevBuf {

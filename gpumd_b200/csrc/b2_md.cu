@@ -223,53 +223,18 @@ int b200md_lj_create(const char* path, int num_atoms, b200md_lj** out)
     set_error("b200md_lj_create: no CUDA device (libb200md has no CPU fallback)");
     return B200MD_ERR_CUDA;
   }
-  FILE* fid = fopen(path, "r");
-  if (!fid) {
-    set_error(std::string("Failed to open ") + path);
-    return B200MD_ERR_IO;
-  }
+  LjFile file;
+  const std::string err = load_lj(path, file);
+  if (!err.empty())
+    return load_error(err);
   b200md_lj* p = new (std::nothrow) b200md_lj;
   if (!p) {
-    fclose(fid);
     set_error("out of host memory");
     return B200MD_ERR_ARG;
   }
-  char name[64];
-  int nt = 0;
-  // "lj Nt sym..." then Nt*Nt lines "epsilon sigma cutoff" (force.cu:93-100, lj.cu:28-56)
-  if (fscanf(fid, "%63s%d", name, &nt) != 2 || std::strcmp(name, "lj") != 0 || nt < 1 || nt > 10) {
-    fclose(fid);
-    delete p;
-    set_error("Incorrect number of LJ parameters.");
-    return B200MD_ERR_ARG;
-  }
-  p->nt = nt;
-  for (int k = 0; k < nt; ++k) {
-    if (fscanf(fid, "%63s", name) != 1) {
-      fclose(fid);
-      delete p;
-      set_error("Reading error for LJ potential.");
-      return B200MD_ERR_ARG;
-    }
-    p->symbols.push_back(name);
-  }
-  std::vector<float> s6(nt * nt), s12(nt * nt), c2(nt * nt);
-  for (int a = 0; a < nt; ++a)
-    for (int b = 0; b < nt; ++b) {
-      double eps, sig, cut;
-      if (fscanf(fid, "%lf%lf%lf", &eps, &sig, &cut) != 3) {
-        fclose(fid);
-        delete p;
-        set_error("Reading error for LJ potential.");
-        return B200MD_ERR_ARG;
-      }
-      s6[a * nt + b] = (float)(std::pow(sig, 6.0) * eps * 4.0);
-      s12[a * nt + b] = (float)(std::pow(sig, 12.0) * eps * 4.0);
-      c2[a * nt + b] = (float)(cut * cut);
-      if (p->rc < cut)
-        p->rc = cut;
-    }
-  fclose(fid);
+  p->nt = file.nt;
+  p->symbols = file.symbols;
+  p->rc = file.rc;
   p->n = num_atoms;
   const size_t N = (size_t)num_atoms;
   int rc = B200MD_OK;
@@ -278,19 +243,11 @@ int b200md_lj_create(const char* path, int num_atoms, b200md_lj** out)
     B2_CUDA(cudaMemcpy(d.p, h.data(), sizeof(float) * h.size(), cudaMemcpyHostToDevice));
     return B200MD_OK;
   };
-  if ((rc = up(p->s6e4, s6)) || (rc = up(p->s12e4, s12)) || (rc = up(p->rc2, c2))) {
+  if ((rc = up(p->s6e4, file.s6e4)) || (rc = up(p->s12e4, file.s12e4)) || (rc = up(p->rc2, file.rc2))) {
     delete p;
     return rc;
   }
-  // neighbor.initialize(rc, num_atoms, 700), lj.cu:58 -> capacity 700*((rc+1)/rc)^3 by default.
-  // B200MD_TIGHT_LISTS=1 bounds it by what rc+skin can hold at twice liquid-argon density (a
-  // memory knob for very large systems; an overflow is still latched and reported).
-  const double rs = p->rc + 1.0;
-  int mn = (int)(700 * rs * rs * rs / (p->rc * p->rc * p->rc));
-  const int mn_dense = (int)(4.19 * rs * rs * rs * 0.06) + 32;
-  if (b2_tight_lists() && mn > mn_dense)
-    mn = mn_dense;
-  if ((rc = p->nb.init(num_atoms, p->rc, mn)) != B200MD_OK) {
+  if ((rc = p->nb.init(num_atoms, p->rc, file.mn_skin)) != B200MD_OK) {
     delete p;
     return rc;
   }
@@ -300,7 +257,7 @@ int b200md_lj_create(const char* path, int num_atoms, b200md_lj** out)
     return B200MD_ERR_CUDA;
   }
   B2LjView& P = p->view;
-  P.nt = nt;
+  P.nt = p->nt;
   P.s6e4 = p->s6e4.p;
   P.s12e4 = p->s12e4.p;
   P.rc2 = p->rc2.p;

@@ -15,6 +15,7 @@
 // run-to-run identical on any device.
 #include "../../include/b200md.h"
 #include "b2_host.h"
+#include "b2_setup.h" // make_box
 #include "b2_reduce.cuh"
 #include <cmath>
 #include <new>

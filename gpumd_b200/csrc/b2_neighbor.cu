@@ -318,20 +318,6 @@ __global__ void k_rebuild_done(int* flags)
 
 } // namespace
 
-B2Grid make_grid(const B2Box& box, double cell_size)
-{
-  B2Grid g;
-  for (int d = 0; d < 3; ++d) {
-    int nb = (int)floor(box.thickness[d] / cell_size);
-    if (nb < 1)
-      nb = 1;
-    g.nb[d] = nb;
-    g.scale[d] = (double)nb;
-  }
-  g.ncell = g.nb[0] * g.nb[1] * g.nb[2];
-  return g;
-}
-
 int Neighbor::init(int num_atoms, double rc_, int mn_skin_)
 {
   n = num_atoms;
@@ -412,22 +398,19 @@ int Neighbor::update(
     if (rc_inv != B200MD_OK)
       return rc_inv;
   }
-  // the cell list needs >= 5 half-(rc+skin) cells per periodic direction.  b200md_nep_compute never
-  // gets here with a thinner box (it evaluates a supercell instead); LJ / Tersoff / EAM do
-  for (int d = 0; d < 3; ++d) {
-    if (box.pbc[d] && box.thickness[d] <= 2.5 * (rc + skin)) {
-      set_error(
-        "periodic box thickness <= 2.5*(rc+1): small boxes are supported for NEP only (supercell "
-        "path); this potential needs a larger box or a replicated cell");
-      return B200MD_ERR_SMALL_BOX;
-    }
+  // b200md_nep_compute never gets here with a thinner box (it evaluates a supercell instead); LJ / Tersoff /
+  // EAM do
+  int reps[3];
+  if (supercell_reps(box, rc, skin, reps) > 1) {
+    set_error(
+      "periodic box thickness <= 2.5*(rc+1): small boxes are supported for NEP only (supercell "
+      "path); this potential needs a larger box or a replicated cell");
+    return B200MD_ERR_SMALL_BOX;
   }
   const B2Grid g = make_grid(box, 0.5 * (rc + skin));
-  for (int d = 0; d < 3; ++d) {
-    if (box.pbc[d] && g.nb[d] < 5) {
-      set_error("internal: fewer than 5 cells in a periodic direction");
-      return B200MD_ERR_SMALL_BOX;
-    }
+  if (grid_too_coarse(box, g)) {
+    set_error("internal: fewer than 5 cells in a periodic direction");
+    return B200MD_ERR_SMALL_BOX;
   }
   if ((size_t)g.ncell + 1 > cell_start.n) {
     const size_t cap = (size_t)(g.ncell * 1.2) + 64;
@@ -506,11 +489,9 @@ int Neighbor::sort_cells(
       return rc_inv;
   }
   const B2Grid g = make_grid(box, cell_size);
-  for (int d = 0; d < 3; ++d) {
-    if (box.pbc[d] && g.nb[d] < 5) {
-      set_error("sort_cells: fewer than 5 cells in a periodic direction (box thinner than 2.5 cutoffs)");
-      return B200MD_ERR_SMALL_BOX;
-    }
+  if (grid_too_coarse(box, g)) {
+    set_error("sort_cells: fewer than 5 cells in a periodic direction (box thinner than 2.5 cutoffs)");
+    return B200MD_ERR_SMALL_BOX;
   }
   if ((size_t)g.ncell + 1 > cell_start.n) {
     const size_t cap = (size_t)(g.ncell * 1.2) + 64;

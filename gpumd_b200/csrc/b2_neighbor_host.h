@@ -2,18 +2,9 @@
 #pragma once
 #include "b2_host.h"
 #include "b2_neighbor.cuh"
-#include <cstdlib>
+#include "b2_setup.h"
 
 namespace b2 {
-
-// B200MD_TIGHT_LISTS=1: size the LJ / EAM skin lists by density instead of the reference's 700 / 400
-inline bool b2_tight_lists()
-{
-  const char* e = getenv("B200MD_TIGHT_LISTS");
-  return e && e[0] == '1';
-}
-
-B2Grid make_grid(const B2Box& box, double cell_size);
 
 class Neighbor
 {

@@ -18,24 +18,8 @@ namespace b2 {
 
 namespace {
 
-constexpr int BLK = 128;
+constexpr int BLK = NEP_BLK;
 constexpr int MLP_BLK = 256;
-// k_angular_fused runs for models with a zero-padded descriptor of 32 (the width whose instances ptxas
-// compiles without spills at three blocks per SM; at 48 every instance spills) and where two of its
-// blocks fit an SM's 228 KB of shared memory (1 KB reserved per block)
-constexpr int FUSED_DIMP = 32;
-constexpr size_t FUSED_MAX_SMEM = 113 * 1024;
-// Angular shapes k_angular_fused is compiled for (B2AngShape): NEP4's default n_max = 4 4 with l_max = 4 2 0
-// (dim 30) and 4 0 0 (dim 25).  Each shape adds 12 instances (NT x K1 x ORTHO, about 15 s of build time);
-// every other shape within the budget runs the run-time-shape instance.
-enum { FUSED_SHAPE_NONE, FUSED_SHAPE_RT, FUSED_SHAPE_4B, FUSED_SHAPE_3B };
-
-int fused_shape_of(const NepModel& m)
-{
-  if (m.nr1 == 5 && m.na1 == 5 && !m.has1111)
-    return m.has222 ? FUSED_SHAPE_4B : FUSED_SHAPE_3B;
-  return FUSED_SHAPE_RT;
-}
 
 __global__ void __launch_bounds__(BLK) k_split(B2NepView P, B2Box box)
 {
@@ -388,28 +372,12 @@ struct b200md_nep {
   DevBuf<int> nn_r, nl_r, nn_a, nl_a;
   DevBuf<int> aslot, nla_rs; // see B2NepView::aslot
   DevBuf<int> arev;          // few-type path: slot of i in the angular list of its m-th angular neighbour
-  bool rev_slot = false;
   DevBuf<float> q, sfx, FpR, FpA, U, f12;
   DevBuf<double> acc;
   DevBuf<float> tc_img, qt, fpt; // tile-major q / dU/dq for k_mlp_tc (B2NepView::qt)
   int num_sms = 132;
-  int tc_ctas_cap = 0;  // B200MD_NEP_TC_CTAS: at most this many CTAs of k_mlp_tc (0: as many as fit)
   int tc_ctas_last = 0; // CTAs of the last k_mlp_tc launch (0: the last compute did not run it)
-  int variant = 0;        // B200MD_NEP_VARIANT: kernel tuning variants for A/B measurements
-  bool fuse_split = false; // many-type path: neighbour split inside the radial descriptor pass
-  bool use_tc = false; // hidden layer on the tensor cores (k_mlp_tc) instead of k_mlp
-  bool ang_fused = false; // k_angular_fused instead of k_desc_angular2 + hidden layer + k_force_angular2
-  int fused_shape = 0;     // its instance: FUSED_SHAPE_* (b200md_nep_info 10)
-  size_t fused_smem = 0;  // its dynamic shared memory per block
-  bool slot_map = false;  // k_force_final2: thread per tile slot (type-pure warps); measured slower
-                          // (H100, 1 M-atom PbTe: 1.26 vs 1.02 ms), B200MD_NEP_SLOTMAP=1 for A/B runs
-  bool rad_direct = false; // many types: contract every pair on the spot (k_desc_radial<-1,...>), see nep_setup
-  bool rad_reg = false;   // 3..16 types: radial accumulators in registers (k_desc_radial<4|8|16,...>); slower
-                          // than the shared-memory accumulators on UNEP-v1, B200MD_NEP_RADREG=1
-  int rad_nt = 0;         // 3+ types: NT of the k_desc_radial instance (-1, 0, 4, 8, 16), see nep_setup
-  bool ang_cstage = true; // k_desc_angular: coefficient table staged in shared memory
-  bool radial_v2 = false; // few-type radial passes of b2_nep_radial.cuh (planes, branch-free loop)
-  bool sched = false;     // their warps follow Neighbor::seg_order (B200MD_NEP_SCHED=0: identity, A/B runs)
+  NepPlan plan;         // kernel paths, switches and budgets (nep_plan)
   // small periodic boxes (SURVEY 8f rank 1): supercell replication, see b200md_nep_compute
   DevBuf<int> rep_type;
   DevBuf<double> rep_pos, rep_out;
@@ -423,8 +391,6 @@ struct b200md_nep {
   double act_lo[3] = {0, 0, 0}, act_hi[3] = {0, 0, 0};
   B2NepView view;
   StageProfiler prof;
-  int ang_block = BLK;
-  size_t ang_smem = 0, rad_smem = 0;
 };
 
 namespace {
@@ -434,10 +400,10 @@ template <int NT, int K1, bool SPLIT>
 int launch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
   auto kern = k_desc_radial<NT, K1, SPLIT>;
-  if (NT == 0 && p->rad_smem > 48 * 1024)
+  if (NT == 0 && p->plan.rad_smem > 48 * 1024)
     B2_CUDA(cudaFuncSetAttribute(
-      kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->rad_smem));
-  kern<<<grid_for(p->n, BLK), BLK, NT == 0 ? p->rad_smem : 0, st>>>(p->view, box);
+      kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->plan.rad_smem));
+  kern<<<grid_for(p->n, BLK), BLK, NT == 0 ? p->plan.rad_smem : 0, st>>>(p->view, box);
   B2_LAUNCHED();
   return B200MD_OK;
 }
@@ -450,7 +416,7 @@ int dispatch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
     k_team_desc_radial<1, K1><<<team_grid, BLK, 0, st>>>(p->view, box);
   } else if (p->view.team) {
     k_team_desc_radial<2, K1><<<team_grid, BLK, 0, st>>>(p->view, box);
-  } else if (p->radial_v2) {
+  } else if (p->plan.radial_v2) {
     const B2NepView& P = p->view;
     B2RadialDescArgs A;
     A.n = P.n; A.nt = P.nt; A.nr1 = P.nr1; A.mn_r = P.mn_r; A.mn_a = P.mn_a;
@@ -479,24 +445,24 @@ int dispatch_desc_radial(const b200md_nep* p, const B2Box& box, cudaStream_t st)
   } else if (p->model.nt == 2) {
     return launch_desc_radial<2, K1, true>(p, box, st);
   } else {
-    // 3+ types: the instance nep_setup chose (p->rad_nt)
-    if (!p->fuse_split) {
+    // 3+ types: the instance nep_plan chose (p->plan.rad_nt)
+    if (!p->plan.fuse_split) {
       k_split<<<grid_for(p->n, BLK), BLK, 0, st>>>(p->view, box);
       B2_LAUNCHED();
     }
-#define B2_DR(NT_)                                                 \
-  return p->fuse_split ? launch_desc_radial<NT_, K1, true>(p, box, st) \
-                       : launch_desc_radial<NT_, K1, false>(p, box, st)
-    if (p->rad_nt == -1)
+#define B2_DR(NT_)                                                          \
+  return p->plan.fuse_split ? launch_desc_radial<NT_, K1, true>(p, box, st) \
+                            : launch_desc_radial<NT_, K1, false>(p, box, st)
+    if (p->plan.rad_nt == -1)
       B2_DR(-1);
-    if (p->rad_nt == 4)
+    if (p->plan.rad_nt == 4)
       B2_DR(4);
     if constexpr (8 * K1 <= 160) {
-      if (p->rad_nt == 8)
+      if (p->plan.rad_nt == 8)
         B2_DR(8);
     }
     if constexpr (16 * K1 <= 160) {
-      if (p->rad_nt == 16)
+      if (p->plan.rad_nt == 16)
         B2_DR(16);
     }
     B2_DR(0);
@@ -511,7 +477,7 @@ int launch_force_final(
   const b200md_nep* p, const B2Box& box, cudaStream_t st, double* pe, double* f, double* v)
 {
   const int g = grid_for(p->n, BLK);
-  switch (p->variant) {
+  switch (p->plan.variant) {
     // B200MD_NEP_VARIANT: register / occupancy variants for A/B runs
     case 1: k_force_final<NT, K1, 6, 1><<<g, BLK, 0, st>>>(p->view, box, pe, f, v); break;
     case 3: k_force_final<NT, K1, 5, 1><<<g, BLK, 0, st>>>(p->view, box, pe, f, v); break;
@@ -537,10 +503,10 @@ int dispatch_force_final(
     k_team_force_final<1, K1><<<team_grid, BLK, 0, st>>>(p->view, box, pe, f, v);
   else if (p->view.team)
     k_team_force_final<2, K1><<<team_grid, BLK, 0, st>>>(p->view, box, pe, f, v);
-  else if (p->radial_v2) {
+  else if (p->plan.radial_v2) {
     // one thread per tile slot when type tiles exist (type-pure warps), else per sorted atom
     B2NepView V = p->view;
-    if (!p->slot_map)
+    if (!p->plan.slot_map)
       V.tile_atom = nullptr; // B200MD_NEP_SLOTMAP=0: thread per sorted atom (A/B runs)
     const int g = V.tile_atom ? p->nb.max_tiles() : grid_for(p->n, BLK);
     const int4* p0 = p->nb.plane0.p;
@@ -552,9 +518,9 @@ int dispatch_force_final(
     // spills 1.30 ms, 4 blocks / 128 regs (variant 2) 1.00 ms, variant 3 1.02 ms
 #define B2_FF2(NT_, ORTHO_)                                                                      \
   do {                                                                                           \
-    if (p->variant == 1)                                                                         \
+    if (p->plan.variant == 1)                                                                         \
       k_force_final2<NT_, K1, ORTHO_, 6><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
-    else if (p->variant == 2)                                                                    \
+    else if (p->plan.variant == 2)                                                                    \
       k_force_final2<NT_, K1, ORTHO_, 4><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
     else                                                                                         \
       k_force_final2<NT_, K1, ORTHO_, 5><<<g, BLK, 0, st>>>(V, p0, p1, pz, ar, box, pe, f, v); \
@@ -598,10 +564,10 @@ int launch_angular2(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool
     return B200MD_OK;
   }
   auto kern = k_force_angular2<NT, K1, ORTHO>;
-  const size_t bytes = p->ang_smem + ctab;
+  const size_t bytes = p->plan.ang_smem + ctab;
   if (bytes > 48 * 1024)
     B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  kern<<<grid_for(p->n, p->ang_block), p->ang_block, bytes, st>>>(p->view, p0, p1, pz, box, p->arev.p);
+  kern<<<grid_for(p->n, p->plan.ang_block), p->plan.ang_block, bytes, st>>>(p->view, p0, p1, pz, box, p->arev.p);
   B2_LAUNCHED();
   return B200MD_OK;
 }
@@ -616,12 +582,12 @@ size_t ang_coeff_bytes(const b200md_nep* p)
 
 // shared-memory copy of the angular coefficients when three blocks of it fit an SM
 // (B200MD_NEP_CSTAGE=0: read them from global memory)
-bool ang_coeff_staged(const b200md_nep* p) { return p->ang_cstage && ang_coeff_bytes(p) <= 72 * 1024; }
+bool ang_coeff_staged(const b200md_nep* p) { return p->plan.ang_cstage && ang_coeff_bytes(p) <= 72 * 1024; }
 
 template <int K1>
 int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool force)
 {
-  if (p->radial_v2) {
+  if (p->plan.radial_v2) {
     if (p->model.nt == 1 && box.ortho)
       return launch_angular2<1, K1, true>(p, box, st, force);
     if (p->model.nt == 1)
@@ -644,14 +610,14 @@ int launch_angular(const b200md_nep* p, const B2Box& box, cudaStream_t st, bool 
     return B200MD_OK;
   }
   void (*kern)(B2NepView, B2Box) = k_force_angular<K1, 128>;
-  if (p->ang_block == 64)
+  if (p->plan.ang_block == 64)
     kern = k_force_angular<K1, 64>;
-  else if (p->ang_block == 32)
+  else if (p->plan.ang_block == 32)
     kern = k_force_angular<K1, 32>;
-  if (p->ang_smem > 48 * 1024)
+  if (p->plan.ang_smem > 48 * 1024)
     B2_CUDA(cudaFuncSetAttribute(
-      kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->ang_smem));
-  kern<<<grid_for(p->n, p->ang_block), p->ang_block, p->ang_smem, st>>>(p->view, box);
+      kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->plan.ang_smem));
+  kern<<<grid_for(p->n, p->plan.ang_block), p->plan.ang_block, p->plan.ang_smem, st>>>(p->view, box);
   B2_LAUNCHED();
   return B200MD_OK;
 }
@@ -660,9 +626,9 @@ template <int NT, int K1, int DIMP, bool ORTHO, class SH>
 int launch_fused_inst(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
   auto kern = k_angular_fused<NT, K1, DIMP, ORTHO, SH>;
-  if (p->fused_smem > 48 * 1024)
-    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->fused_smem));
-  kern<<<grid_for(p->n, BLK), BLK, p->fused_smem, st>>>(
+  if (p->plan.fused_smem > 48 * 1024)
+    B2_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->plan.fused_smem));
+  kern<<<grid_for(p->n, BLK), BLK, p->plan.fused_smem, st>>>(
     p->view, p->nb.plane0.p, p->nb.plane1.p, p->nb.planez.p, box, p->arev.p);
   B2_LAUNCHED();
   return B200MD_OK;
@@ -678,12 +644,12 @@ int launch_fused_shape(const b200md_nep* p, const B2Box& box, cudaStream_t st)
                    : launch_fused_inst<2, K1, FUSED_DIMP, false, SH>(p, box, st);
 }
 
-// the one hidden-layer width k_angular_fused is instantiated for (FUSED_DIMP, see nep_setup), on the angular
-// shape p->fused_shape (fused_shape_of)
+// the one hidden-layer width k_angular_fused is instantiated for (FUSED_DIMP, see nep_plan), on the angular
+// shape p->plan.fused_shape (fused_shape_of)
 template <int K1>
 int launch_angular_fused(const b200md_nep* p, const B2Box& box, cudaStream_t st)
 {
-  switch (p->fused_shape) {
+  switch (p->plan.fused_shape) {
     case FUSED_SHAPE_4B: return launch_fused_shape<K1, B2AngShape<5, 5, true, false>>(p, box, st);
     case FUSED_SHAPE_3B: return launch_fused_shape<K1, B2AngShape<5, 5, false, false>>(p, box, st);
     default: return launch_fused_shape<K1, B2AngShapeRT>(p, box, st);
@@ -741,7 +707,7 @@ int angular_stages(b200md_nep* p, const B2Box& box, cudaStream_t st)
   }
   pf.end(st, ST_DESC_A);
   pf.begin(st, ST_MLP);
-  if (p->use_tc) {
+  if (p->plan.use_tc) {
     const size_t bytes = b2_tc_smem_bytes(p->model.tc_img_floats, p->model.HN, p->model.DK, p->model.DN,
                                           p->view.N3 ? p->model.K3 : 0);
     if (bytes > 48 * 1024)
@@ -753,8 +719,8 @@ int angular_stages(b200md_nep* p, const B2Box& box, cudaStream_t st)
     per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
     const int tiles = p->nb.max_tiles();
     int ctas = tiles < p->num_sms * per_sm ? tiles : p->num_sms * per_sm;
-    if (p->tc_ctas_cap > 0 && ctas > p->tc_ctas_cap)
-      ctas = p->tc_ctas_cap; // every tile is still computed by one CTA with the same arithmetic
+    if (p->plan.tc_ctas_cap > 0 && ctas > p->plan.tc_ctas_cap)
+      ctas = p->plan.tc_ctas_cap; // every tile is still computed by one CTA with the same arithmetic
     p->tc_ctas_last = ctas;
     k_mlp_tc<<<ctas, 128, bytes, st>>>(p->view);
     B2_LAUNCHED();
@@ -769,7 +735,7 @@ int angular_stages(b200md_nep* p, const B2Box& box, cudaStream_t st)
     case 112: B2_TRY(launch_mlp<112>(p, st)); break;
     default: B2_TRY(launch_mlp<128>(p, st)); break;
   }
-  if (!(p->use_tc && p->view.N3)) { // otherwise k_mlp_tc produced the U table as its third GEMM
+  if (!(p->plan.use_tc && p->view.N3)) { // otherwise k_mlp_tc produced the U table as its third GEMM
     switch (p->model.K1R) {
       case 9: k_utable<9><<<grid_for(n, BLK), BLK, 0, st>>>(p->view); break;
       case 13: k_utable<13><<<grid_for(n, BLK), BLK, 0, st>>>(p->view); break;
@@ -800,7 +766,7 @@ int nep_pipeline(
     default: B2_TRY(dispatch_desc_radial<17>(p, box, st)); break;
   }
   pf.end(st, ST_DESC_R);
-  if (p->ang_fused) {
+  if (p->plan.ang_fused) {
     pf.begin(st, ST_ANG_FUSED);
     switch (p->model.K1A) {
       case 9: B2_TRY(launch_angular_fused<9>(p, box, st)); break;
@@ -846,110 +812,48 @@ int nep_setup(b200md_nep* p, int num_atoms)
   std::vector<float> cov(COVALENT_RADIUS, COVALENT_RADIUS + 94);
   B2_TRY(upload(p->cov_radius, cov));
 
-  // Neighbor::initialize: skin-list capacity MN*((rc+skin)/rc)^3, neighbor.cu:824-829
-  const double rc = m.rc_radial_max;
-  const double rs = rc + 1.0;
-  const int mn_skin = (int)(m.MN_radial * rs * rs * rs / (rc * rc * rc));
-  // radial passes: thread per atom by default.  B200MD_NEP_TEAM=1 selects the lane-team kernels
-  // for one- and two-type models: they cut the L1 gather wavefronts ~3x but cost ~30% more
-  // instructions and are slower.
-  const char* team_env = std::getenv("B200MD_NEP_TEAM");
-  const bool team = m.nt <= 2 && team_env && std::strcmp(team_env, "1") == 0;
-  p->nb.skin_row_major = team;
-  if (const char* v = std::getenv("B200MD_NEP_VARIANT"))
-    p->variant = std::atoi(v);
-  // fused split pays when few skin candidates fail the radial test: (rc+skin)^3 / rc^3 small
-  p->fuse_split = rs * rs * rs / (rc * rc * rc) < 1.45;
-  B2_TRY(p->nb.init(num_atoms, rc, mn_skin));
-  // one- and two-type models: the plane-based radial kernels (B200MD_NEP_RADIAL=v1 keeps the
-  // round-1 kernels for A/B runs)
-  const char* rad_env = std::getenv("B200MD_NEP_RADIAL");
-  p->radial_v2 = m.nt <= 2 && !team && !(rad_env && std::strcmp(rad_env, "v1") == 0) &&
-                 (double)num_atoms * (mn_skin + 2) < 4.0e9; // 32-bit list offsets in those kernels
-  if (const char* v = std::getenv("B200MD_NEP_SLOTMAP"))
-    p->slot_map = std::atoi(v) != 0;
-  if (const char* v = std::getenv("B200MD_NEP_RADREG"))
-    p->rad_reg = std::atoi(v) != 0;
-  if (const char* v = std::getenv("B200MD_NEP_CSTAGE"))
-    p->ang_cstage = std::atoi(v) != 0;
-  p->nb.tag_types = p->radial_v2; // skin entries carry the neighbour type (b2_nep_radial.cuh)
-  // Hidden layer and angular stages.  B200MD_NEP_MLP unset: k_angular_fused where the model fits its budget
-  // (FUSED_DIMP, FUSED_MAX_SMEM; DESIGN.md 3.2); then the SIMT layer is also the hidden layer of the
-  // generic kernels (B200MD_NEP_RADIAL=v1), which keeps the two paths bit-identical.  Otherwise the
-  // tensor cores unless the shapes do not fit them.  B200MD_NEP_MLP=simt / =tc select the SIMT / the
-  // tensor-core layer between separate angular kernels.
-  const char* mlp_env = std::getenv("B200MD_NEP_MLP");
-  const bool mlp_simt = mlp_env && std::strcmp(mlp_env, "simt") == 0;
-  p->fused_smem = b2_fused_smem_bytes(m.nt, m.na1, m.K1A, m.nneu, m.DIMP);
-  const bool fused_fits = m.nt <= 2 && !mlp_env && m.DIMP == FUSED_DIMP &&
-                          p->fused_smem <= FUSED_MAX_SMEM;
-  p->ang_fused = fused_fits && p->radial_v2;
-  p->fused_shape = p->ang_fused ? fused_shape_of(m) : FUSED_SHAPE_NONE;
-  p->use_tc = m.tc_ok && !mlp_simt && !fused_fits;
-  if (p->radial_v2)
-    B2_TRY(p->nb.enable_planes());
-  {
-    const char* e = std::getenv("B200MD_NEP_SCHED");
-    p->sched = p->radial_v2 && !(e && e[0] == '0');
-    if (p->sched)
-      B2_TRY(p->nb.enable_schedule());
+  const std::string err = nep_plan(m, num_atoms, p->plan);
+  if (!err.empty()) {
+    set_error(err);
+    return B200MD_ERR_ARG;
   }
-  const int pitch_r = (m.MN_radial + 7) / 8 * 8;
-  // B200MD_NEP_REVSLOT=1 (many types with the neighbour split as its own kernel): direct reverse slots
-  // for the angular pair reduction instead of a binary search per pair: k_force_final gets faster on
-  // UNEP-v1, but the extra stores slow k_split down by more, so it stays an opt-in.
-  {
-    const char* e = std::getenv("B200MD_NEP_REVSLOT");
-    p->rev_slot = m.nt > 2 && !team && !p->fuse_split && e && e[0] == '1';
-    if (p->rev_slot) {
-      B2_TRY(p->nb.enable_reverse());
-      B2_CUDA(p->aslot.reserve(N * (size_t)mn_skin));
-      B2_CUDA(p->nla_rs.reserve(N * (size_t)m.MN_angular));
-      B2_CUDA(cudaMemset(p->aslot.p, 0xff, sizeof(int) * N * (size_t)mn_skin));
-      B2_CUDA(cudaMemset(p->nla_rs.p, 0, sizeof(int) * N * (size_t)m.MN_angular));
-    }
+  const NepPlan& plan = p->plan;
+  if (plan.debug_skip)
+    fprintf(stderr, "libb200md: B200MD_DEBUG_SKIP=%d -- parts of the NEP force are SWITCHED OFF "
+                    "(kernel timing only, results are wrong)\n", plan.debug_skip);
+  p->nb.skin_row_major = plan.team;
+  B2_TRY(p->nb.init(num_atoms, m.rc_radial_max, plan.mn_skin));
+  p->nb.tag_types = plan.radial_v2; // skin entries carry the neighbour type (b2_nep_radial.cuh)
+  if (plan.radial_v2)
+    B2_TRY(p->nb.enable_planes());
+  if (plan.sched)
+    B2_TRY(p->nb.enable_schedule());
+  if (plan.rev_slot) {
+    B2_TRY(p->nb.enable_reverse());
+    B2_CUDA(p->aslot.reserve(N * (size_t)plan.mn_skin));
+    B2_CUDA(p->nla_rs.reserve(N * (size_t)m.MN_angular));
+    B2_CUDA(cudaMemset(p->aslot.p, 0xff, sizeof(int) * N * (size_t)plan.mn_skin));
+    B2_CUDA(cudaMemset(p->nla_rs.p, 0, sizeof(int) * N * (size_t)m.MN_angular));
   }
 
   B2_CUDA(p->nn_r.reserve(N));
-  B2_CUDA(p->nl_r.reserve(N * (size_t)pitch_r));
+  B2_CUDA(p->nl_r.reserve(N * (size_t)plan.pitch_r));
   B2_CUDA(p->nn_a.reserve(N));
   B2_CUDA(p->nl_a.reserve(N * m.MN_angular));
   B2_CUDA(p->q.reserve(N * m.dim));
-  if (!p->ang_fused) { // k_angular_fused keeps s and dU/dq on chip
+  if (!plan.ang_fused) { // k_angular_fused keeps s and dU/dq on chip
     B2_CUDA(p->sfx.reserve(N * m.na1 * B2_NABC));
     B2_CUDA(p->FpR.reserve(N * m.nr1));
     B2_CUDA(p->FpA.reserve(N * m.dim_angular));
   }
   B2_CUDA(p->U.reserve(N * m.UST));
-  B2_CUDA(p->f12.reserve(N * (p->radial_v2 ? 4 : 3) * m.MN_angular)); // few types: float4 entries
-  if (p->radial_v2)
+  B2_CUDA(p->f12.reserve(N * (plan.radial_v2 ? 4 : 3) * m.MN_angular)); // few types: float4 entries
+  if (plan.radial_v2)
     B2_CUDA(p->arev.reserve(N * m.MN_angular));
   B2_CUDA(p->acc.reserve(N)); // site energies from the MLP pass
 
   B2NepView& P = p->view;
-  std::memset(&P, 0, sizeof P);
-  P.nt = m.nt;
-  P.nr1 = m.nr1;
-  P.na1 = m.na1;
-  P.kr1 = m.kr1;
-  P.ka1 = m.ka1;
-  P.K1R = m.K1R;
-  P.K1A = m.K1A;
-  P.KP = m.KP;
-  P.UST = m.UST;
-  P.has222 = m.has222;
-  P.has1111 = m.has1111;
-  P.num_L = m.num_L;
-  P.dim = m.dim;
-  P.dim_ang = m.dim_angular;
-  P.nneu = m.nneu;
-  P.DIMP = m.DIMP;
-  P.zbl_enabled = m.zbl_enabled;
-  P.zbl_flexible = m.zbl_flexible;
-  P.zbl_typewise = m.zbl_typewise;
-  P.zbl_rc_inner = m.zbl_rc_inner;
-  P.zbl_rc_outer = m.zbl_rc_outer;
-  P.zbl_typewise_factor = m.zbl_typewise_factor;
+  P = nep_view(m, plan, num_atoms);
   P.rc_r = p->rc_r.p;
   P.rcinv_r = p->rcinv_r.p;
   P.rc2_r = p->rc2_r.p;
@@ -958,21 +862,8 @@ int nep_setup(b200md_nep* p, int num_atoms)
   P.rc2_a = p->rc2_a.p;
   P.c_r = p->c_r.p;
   P.c_a = p->c_a.p;
-  {
-    // B200MD_NEP_CVEC=0: scalar coefficient loads in the radial contraction (A/B switch; results are
-    // bit-identical).  The angular kernels always use the padded rows.
-    const char* e = getenv("B200MD_NEP_CVEC");
-    const bool cvec = !(e && e[0] == '0');
-    P.c_a4 = reinterpret_cast<const float4*>(p->c_a4.p);
-    P.c_r4 = cvec ? reinterpret_cast<const float4*>(p->c_r4.p) : nullptr;
-    P.nqr = m.nqr;
-    if (const char* d = getenv("B200MD_DEBUG_SKIP")) {
-      P.debug_skip = atoi(d);
-      if (P.debug_skip)
-        fprintf(stderr, "libb200md: B200MD_DEBUG_SKIP=%d -- parts of the NEP force are SWITCHED OFF "
-                        "(kernel timing only, results are wrong)\n", P.debug_skip);
-    }
-  }
+  P.c_a4 = reinterpret_cast<const float4*>(p->c_a4.p);
+  P.c_r4 = plan.c_r4 ? reinterpret_cast<const float4*>(p->c_r4.p) : nullptr;
   P.w0p = p->w0p.p;
   P.b0 = p->b0.p;
   P.w1 = p->w1.p;
@@ -981,44 +872,36 @@ int nep_setup(b200md_nep* p, int num_atoms)
   P.zbl_z = p->zbl_z.p;
   P.zbl_para = p->zbl_para.p;
   P.cov_radius = p->cov_radius.p;
-  P.n = num_atoms;
-  P.mn_r = m.MN_radial;
-  P.mn_a = m.MN_angular;
   P.atoms = p->nb.atoms.p;
   P.perm = p->nb.perm.p;
   P.nn_skin = p->nb.nn_skin.p;
   P.nl_skin = p->nb.nl_skin.p;
-  P.rskin = p->rev_slot ? p->nb.rskin.p : nullptr;
-  P.aslot = p->rev_slot ? p->aslot.p : nullptr;
-  P.nla_rs = p->rev_slot ? p->nla_rs.p : nullptr;
+  P.rskin = plan.rev_slot ? p->nb.rskin.p : nullptr;
+  P.aslot = plan.rev_slot ? p->aslot.p : nullptr;
+  P.nla_rs = plan.rev_slot ? p->nla_rs.p : nullptr;
   P.nn_r = p->nn_r.p;
   P.nl_r = p->nl_r.p;
   P.nn_a = p->nn_a.p;
   P.nl_a = p->nl_a.p;
   P.q = p->q.p;
-  P.sfx = p->ang_fused ? nullptr : p->sfx.p;
-  P.FpR = p->ang_fused ? nullptr : p->FpR.p;
-  P.FpA = p->ang_fused ? nullptr : p->FpA.p;
+  P.sfx = plan.ang_fused ? nullptr : p->sfx.p;
+  P.FpR = plan.ang_fused ? nullptr : p->FpR.p;
+  P.FpA = plan.ang_fused ? nullptr : p->FpA.p;
   P.U = p->U.p;
   P.f12 = p->f12.p;
   P.acc = p->acc.p;
   P.flags = p->nb.flags.p;
-  P.seg_order = p->sched ? p->nb.seg_order.p : nullptr;
-  P.team = team ? 1 : 0;
-  P.u_planes = p->radial_v2 ? 2 : (team ? 1 : 0);
-  P.pitch_r = pitch_r;
+  P.seg_order = plan.sched ? p->nb.seg_order.p : nullptr;
+  P.u_planes = plan.radial_v2 ? 2 : (plan.team ? 1 : 0);
   {
     const B2NeighborView nv = p->nb.view();
     P.skin_si = nv.skin_si;
     P.skin_sk = nv.skin_sk;
   }
-  if (p->use_tc) {
+  if (plan.use_tc) {
     int dev = 0;
     B2_CUDA(cudaGetDevice(&dev));
     B2_CUDA(cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, dev));
-    // B200MD_NEP_TC_CTAS=k (tests): cap the persistent CTAs so that each walks many tiles
-    if (const char* e = std::getenv("B200MD_NEP_TC_CTAS"))
-      p->tc_ctas_cap = std::atoi(e) > 0 ? std::atoi(e) : 0;
     B2_TRY(p->nb.enable_type_tiles(m.nt));
     B2_TRY(upload(p->tc_img, m.tc_img));
     P.tc_img = p->tc_img.p;
@@ -1028,8 +911,7 @@ int nep_setup(b200md_nep* p, int num_atoms)
     P.DN = m.DN;
     P.K3 = m.K3;
     // the U table as a third GEMM of the same kernel (AoS rows or float4 planes, see epilogue 3)
-    const char* u_env = std::getenv("B200MD_NEP_UTABLE");
-    P.N3 = (m.tc3_ok && !(u_env && std::strcmp(u_env, "simt") == 0)) ? m.N3 : 0;
+    P.N3 = plan.utable_tc ? m.N3 : 0;
     P.tile_atom = p->nb.tile_atom.p;
     { // tile-major q and dU/dq: zeroed once so that padding rows / columns hold finite values
       const size_t floats = (size_t)p->nb.max_tiles() * 128 * m.DK;
@@ -1045,41 +927,6 @@ int nep_setup(b200md_nep* p, int num_atoms)
     P.tile_type = p->nb.tile_type.p;
     P.tile_meta = p->nb.tile_meta.p;
   }
-
-  // shared-memory budgets
-  // (k_force_angular2: one padded row of b2_ang_ws4(na1) float4s per thread)
-  const size_t ang_row = p->radial_v2 ? b2_ang_ws4(m.na1) * sizeof(float4) : m.na1 * B2_NABC * sizeof(float);
-  p->ang_block = BLK;
-  p->ang_smem = ang_row * p->ang_block;
-  while (p->ang_smem > 200 * 1024 && p->ang_block > 32) {
-    p->ang_block /= 2;
-    p->ang_smem = ang_row * p->ang_block;
-  }
-  // Radial descriptor of a many-type model: per-type accumulators in shared memory while two blocks of
-  // them fit an SM, else (NEP89: 89 species) the per-pair contraction, which needs no such storage.
-  // B200MD_NEP_RADDIRECT=1 forces the latter for any model with more than two types (tests, A/B).
-  p->rad_smem = (size_t)m.nt * m.K1R * BLK * sizeof(float);
-  p->rad_direct = false;
-  if (m.nt > 2) {
-    const char* e = std::getenv("B200MD_NEP_RADDIRECT");
-    const bool forced = e && e[0] == '1';
-    if (forced || p->rad_smem > 96 * 1024) {
-      if (m.nqr > B2_NQMAX) {
-        set_error("n_max_radial above 19 is not supported for models with this many atom types");
-        return B200MD_ERR_ARG;
-      }
-      p->rad_direct = true;
-      p->rad_smem = 0;
-      P.c_r4 = reinterpret_cast<const float4*>(p->c_r4.p); // regardless of B200MD_NEP_CVEC
-    }
-  }
-  // 3..16 types: register accumulators (B200MD_NEP_RADREG=1) when NT*K1 fits the register file; the
-  // default keeps the accumulators in shared memory
-  {
-    const int nt = m.nt;
-    const int ntb = !p->rad_reg ? 0 : nt <= 4 ? 4 : nt <= 8 ? 8 : nt <= 16 ? 16 : 0;
-    p->rad_nt = p->rad_direct ? -1 : ntb * m.K1R <= 160 ? ntb : 0;
-  }
   B2_CUDA(cudaDeviceSynchronize());
   return B200MD_OK;
 }
@@ -1087,7 +934,7 @@ int nep_setup(b200md_nep* p, int num_atoms)
 // type tiles of the last list rebuild (synchronises; 0 without tiles)
 int nep_tile_count(const b200md_nep* p)
 {
-  if (!p->use_tc || !p->nb.have_grid)
+  if (!p->plan.use_tc || !p->nb.have_grid)
     return 0;
   int ntile = 0;
   if (cudaDeviceSynchronize() != cudaSuccess ||
@@ -1118,10 +965,8 @@ int b200md_nep_create(const char* path, int num_atoms, b200md_nep** out)
   }
   const std::string err = p->model.load(path);
   if (!err.empty()) {
-    set_error(err);
-    const bool io = err.rfind("Failed to open", 0) == 0;
     delete p;
-    return io ? B200MD_ERR_IO : B200MD_ERR_ARG;
+    return load_error(err);
   }
   const int rc = nep_setup(p, num_atoms);
   if (rc != B200MD_OK) {
@@ -1148,35 +993,35 @@ int b200md_nep_info(const b200md_nep* p, int what)
       const_cast<b200md_nep*>(p)->nb.check(0, &bits, &rebuilds);
       return rebuilds;
     }
-    case 7: return p->sched ? p->nb.num_segments() : 0;
+    case 7: return p->plan.sched ? p->nb.num_segments() : 0;
     case 8: return nep_tile_count(p);
     case 9: return p->tc_ctas_last;
-    case 10: return p->fused_shape;
-    case 11: return p->ang_fused ? 0 : p->ang_block;
+    case 10: return p->plan.fused_shape;
+    case 11: return p->plan.ang_fused ? 0 : p->plan.ang_block;
     case 12: { // mirrors dispatch_desc_radial
       const int nt = p->model.nt;
       if (p->view.team)
         return 200 + nt;
-      if (p->radial_v2)
+      if (p->plan.radial_v2)
         return 100 + nt;
-      return nt <= 2 ? nt : p->rad_nt;
+      return nt <= 2 ? nt : p->plan.rad_nt;
     }
     case 13:
-      if (p->view.team || p->radial_v2)
+      if (p->view.team || p->plan.radial_v2)
         return -1;
-      return (p->model.nt <= 2 || p->fuse_split) ? 1 : 0;
+      return (p->model.nt <= 2 || p->plan.fuse_split) ? 1 : 0;
     case 14:
-      if (p->ang_fused)
+      if (p->plan.ang_fused)
         return 0;
-      return (p->use_tc && p->view.N3) ? 1 : 2;
+      return (p->plan.use_tc && p->view.N3) ? 1 : 2;
     case 15:
-      if (p->radial_v2)
+      if (p->plan.radial_v2)
         return -1;
       return ang_coeff_staged(p) ? 1 : 0;
-    case 16: return p->rev_slot ? 1 : 0;
-    case 17: return (p->ang_fused || p->use_tc) ? 0 : p->model.DIMP;
+    case 16: return p->plan.rev_slot ? 1 : 0;
+    case 17: return (p->plan.ang_fused || p->plan.use_tc) ? 0 : p->model.DIMP;
     case 18:
-      if (p->ang_fused || p->use_tc)
+      if (p->plan.ang_fused || p->plan.use_tc)
         return -1;
       return mlp_weights_staged(p) ? 1 : 0;
     default: return -1;
@@ -1207,12 +1052,8 @@ int b200md_nep_compute(
   // images at 2.5*rc, nep.cu:1304-1312, nep_small_box.cuh): evaluate the smallest supercell that
   // the cell-list path accepts and keep the first replica.  Every atom of that replica sees each
   // periodic image of its neighbours as a distinct atom, exactly the reference's pair set.
-  int reps[3] = {1, 1, 1};
-  const double need = 2.5 * (p->nb.rc + p->nb.skin);
-  for (int d = 0; d < 3; ++d)
-    if (box.pbc[d] && box.thickness[d] <= need)
-      reps[d] = (int)std::floor(need / box.thickness[d]) + 1;
-  const long long R = (long long)reps[0] * reps[1] * reps[2];
+  int reps[3];
+  const long long R = supercell_reps(box, p->nb.rc, p->nb.skin, reps);
   p->rep_n = 0;
   if (R > 1) {
     if (R * n > 50000000LL) {
@@ -1303,13 +1144,13 @@ int b200md_nep_export_neighbors(
       n, p->rep_n ? p->rep_n : n, p->nb.perm.p, p->nn_r.p, p->nl_r.p,
       p->view.team ? (size_t)p->view.pitch_r : 1,
       p->view.team ? 1 : (size_t)n, mn_r, d_NN_r, d_NL_r, p->nb.flags.p,
-      p->radial_v2 ? B2_TAG_MASK : -1);
+      p->plan.radial_v2 ? B2_TAG_MASK : -1);
     B2_LAUNCHED();
   }
   if (d_NN_a && d_NL_a) {
     k_export_list<<<grid_for(n, 128), 128, 0, st>>>(
       n, p->rep_n ? p->rep_n : n, p->nb.perm.p, p->nn_a.p, p->nl_a.p, 1, (size_t)n, mn_a, d_NN_a,
-      d_NL_a, p->nb.flags.p, p->radial_v2 ? B2_TAG_MASK : -1);
+      d_NL_a, p->nb.flags.p, p->plan.radial_v2 ? B2_TAG_MASK : -1);
     B2_LAUNCHED();
   }
   return B200MD_OK;
@@ -1356,7 +1197,7 @@ int b200md_nep_export_descriptors(b200md_nep* p, float* d_q, void* stream)
 int b200md_nep_export_schedule(
   b200md_nep* p, int dims[6], int* d_seg_order, int* d_cell_start, void* stream)
 {
-  if (!p->sched || !p->nb.have_grid) {
+  if (!p->plan.sched || !p->nb.have_grid) {
     set_error("b200md_nep_export_schedule: no schedule (identity schedule, or no compute call yet)");
     return B200MD_ERR_ARG;
   }
@@ -1397,7 +1238,7 @@ int b200md_nep_export_tiles(b200md_nep* p, int* d_slot, int* d_tile_type, void* 
 
 int b200md_nep_export_mlp(b200md_nep* p, float* d_fp, float* d_u, void* stream)
 {
-  if (p->ang_fused) {
+  if (p->plan.ang_fused) {
     set_error("b200md_nep_export_mlp: k_angular_fused keeps dU/dq and the U table on chip");
     return B200MD_ERR_ARG;
   }

@@ -45,6 +45,17 @@
 #define B2_C5B2 (0.026596810706114f)
 
 constexpr int B2_NABC = 24;      // (L_max+1)^2 - 1 for L_max = 4
+constexpr int B2_ABC4 = B2_NABC / 4; // float4 groups of one angular channel
+
+// Shared-memory rows of the few-type angular kernels (b2_nep_angular.cuh): WS4 float4s of per-atom weights
+// per thread, and k_angular_fused's w0 stride and its whole dynamic shared memory per 128-thread block
+B2_HOST_DEVICE constexpr int b2_ang_ws4(int na1) { return B2_ABC4 * na1 + 1; }
+B2_HOST_DEVICE constexpr int b2_fused_w0_stride4(int nneu, int dimp) { return (nneu * dimp / 4) | 1; }
+B2_HOST_DEVICE constexpr size_t b2_fused_smem_bytes(int nt, int na1, int k1a, int nneu, int dimp)
+{
+  return (size_t)128 * b2_ang_ws4(na1) * 16 + (size_t)nt * nt * na1 * ((k1a + 3) / 4) * 16 +
+         (size_t)nt * b2_fused_w0_stride4(nneu, dimp) * 16 + (size_t)2 * nt * nneu * 4;
+}
 
 // list entry = neighbour index | type << 30 (B2NeighborView::tag_types; the radial and angular lists
 // of the few-type kernels in b2_nep_radial.cuh / b2_nep_angular.cuh)

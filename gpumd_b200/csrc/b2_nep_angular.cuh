@@ -17,14 +17,12 @@
 //     directly instead of walking a binary search of dependent loads;
 //   * k_angular_fused runs the descriptor, the hidden layer, the U table and the partial forces of one
 //     atom in one thread, so s, dU/dq and the weights never leave the SM (the default where the model
-//     fits it, see nep_setup); the two-kernel pair with k_mlp / k_mlp_tc in between stays for the models
+//     fits it, see nep_plan); the two-kernel pair with k_mlp / k_mlp_tc in between stays for the models
 //     that do not fit and for B200MD_NEP_MLP=simt / tc.  All of them call the same bodies below.
 #pragma once
 #include "b2_nep_radial.cuh"
 
 namespace b2 {
-
-constexpr int B2_ABC4 = B2_NABC / 4; // float4 groups of one angular channel
 
 // Shape of the angular model: nr1 radial and na1 angular channels, the 4-body (has222) and 5-body
 // (has1111) invariant blocks.  NA1 = 0 reads all four from the model at run time; otherwise they are
@@ -202,8 +200,6 @@ __global__ void __launch_bounds__(128, 3) k_desc_angular2(
 // WS4 = 6*na1 + 1 float4s (the per-atom weights; the odd row stride keeps the 128-bit accesses of a
 // quarter warp on distinct banks), then the coefficient table.
 // ---------------------------------------------------------------------------------------------
-__host__ __device__ constexpr int b2_ang_ws4(int na1) { return B2_ABC4 * na1 + 1; }
-
 // The pair loop of sorted atom i (record a1): w = its row of weights dU/ds[n][abc] (float4 group
 // n*6 + abc/4), ctab_s the staged coefficient table.
 template <int NT, int K1, bool ORTHO, class SH>
@@ -401,7 +397,7 @@ __global__ void __launch_bounds__(128, 3) k_force_angular2(
 
 // ---------------------------------------------------------------------------------------------
 // k_angular_fused: descriptor, hidden layer, U table and angular partial forces of one sorted atom in
-// one thread, for models that fit its budget (b2_fused_smem_bytes, DIMP = 32; nep_setup).  Nothing in
+// one thread, for models that fit its budget (b2_fused_smem_bytes, DIMP = 32; nep_plan).  Nothing in
 // the chain depends on another atom's result, so s[n][abc], dU/dq and dU/ds stay on the SM:
 //   1. descriptor (b2_ang_desc_atom): s goes to the thread's shared-memory row, the angular components
 //      of q to the SoA columns P.q (they stay observable, b200md_nep_export_descriptors);
@@ -419,8 +415,6 @@ __global__ void __launch_bounds__(128, 3) k_force_angular2(
 // type at a stride of b2_fused_w0_stride4 float4s (odd: a warp holding both types reads the two rows
 // on distinct banks), b0 and w1.
 // ---------------------------------------------------------------------------------------------
-__host__ __device__ constexpr int b2_fused_w0_stride4(int nneu, int dimp) { return (nneu * dimp / 4) | 1; }
-
 #ifdef B2_FUSED_STOP
 // Diagnostic builds only (build_lib(variant=..., defs=["B2_FUSED_STOP=k"])): k_angular_fused returns after
 // step k (1 descriptor, 2 hidden layer, 3 U table, 4 weights) so that the stage profiler times the steps
@@ -438,12 +432,6 @@ __host__ __device__ constexpr int b2_fused_w0_stride4(int nneu, int dimp) { retu
 #else
 #define B2_FUSED_MAYBE_STOP(k, ...)
 #endif
-
-__host__ __device__ constexpr size_t b2_fused_smem_bytes(int nt, int na1, int k1a, int nneu, int dimp)
-{
-  return (size_t)128 * b2_ang_ws4(na1) * 16 + (size_t)nt * nt * na1 * ((k1a + 3) / 4) * 16 +
-         (size_t)nt * b2_fused_w0_stride4(nneu, dimp) * 16 + (size_t)2 * nt * nneu * 4;
-}
 
 template <int NT, int K1, int DIMP, bool ORTHO, class SH>
 __global__ void __launch_bounds__(128, 3) k_angular_fused(

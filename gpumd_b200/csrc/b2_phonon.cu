@@ -21,6 +21,7 @@
 // dim = 96.  Eigenvalues come out in ascending order, eigenvectors as columns of a column-major matrix.
 #include "../../include/b200md.h"
 #include "b2_host.h"
+#include "b2_setup.h" // make_box
 #include <cfloat>
 #include <cmath>
 #include <new>

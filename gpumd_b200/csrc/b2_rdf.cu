@@ -179,11 +179,7 @@ int b200md_rdf_create(
     return B200MD_ERR_ARG;
   }
   b200md_rdf* p = new b200md_rdf;
-  p->para.num_bins = num_bins;
-  p->para.num_types = num_types;
-  p->para.num_pairs = num_types * (num_types + 1) / 2;
-  p->para.dr = rc / num_bins;  // rdf.cu:326
-  p->para.rc2 = rc * rc;       // rdf.cu:325
+  p->para = rdf_para(rc, num_bins, num_types);
   p->rc = rc;
   p->n = n;
   p->type_index.assign(type_index, type_index + num_types);

@@ -47,24 +47,6 @@ __global__ void __launch_bounds__(256) k_heat(
     b2_body_heat(i, stride, w, v, heat, hstride);
 }
 
-void fill(B2TersoffPara& t, const double* p)
-{
-  t.a = p[0];
-  t.b = p[1];
-  t.lambda = p[2];
-  t.mu = p[3];
-  t.beta = p[4];
-  t.n = p[5];
-  t.c2 = p[6] * p[6];
-  t.d2 = p[7] * p[7];
-  t.h = p[8];
-  t.r1 = p[9];
-  t.r2 = p[10];
-  t.one_plus = 1.0 + t.c2 / t.d2;
-  t.pi_factor = 3.14159265358979 / (t.r2 - t.r1); // PI, src/utilities/common.cuh:19
-  t.mhn = -0.5 / p[5];
-}
-
 } // namespace
 } // namespace b2
 
@@ -100,73 +82,21 @@ int b200md_tersoff_create(const char* path, int num_atoms, b200md_tersoff** out)
     set_error("b200md_tersoff_create: no CUDA device (libb200md has no CPU fallback)");
     return B200MD_ERR_CUDA;
   }
-  FILE* fid = fopen(path, "r");
-  if (!fid) {
-    set_error(std::string("Failed to open ") + path);
-    return B200MD_ERR_IO;
-  }
-  char name[64];
-  int nt = 0;
-  if (fscanf(fid, "%63s%d", name, &nt) != 2 || std::strcmp(name, "tersoff_1989") != 0 || nt < 1 ||
-      nt > 2) {
-    fclose(fid);
-    set_error("tersoff_1989 potential file: first line must be 'tersoff_1989 <1|2> <symbols>'");
-    return B200MD_ERR_ARG;
-  }
+  TersoffFile file;
+  const std::string err = load_tersoff(path, file);
+  if (!err.empty())
+    return load_error(err);
   b200md_tersoff* p = new (std::nothrow) b200md_tersoff;
   if (!p) {
-    fclose(fid);
     set_error("out of host memory");
     return B200MD_ERR_ARG;
   }
-  p->nt = nt;
-  for (int k = 0; k < nt; ++k) {
-    if (fscanf(fid, "%63s", name) != 1) {
-      fclose(fid);
-      delete p;
-      set_error("Reading error for Tersoff-1989 potential.");
-      return B200MD_ERR_ARG;
-    }
-    p->symbols.push_back(name);
-  }
-  double para[23] = {0};
-  const int want = nt == 1 ? 11 : 23;
-  for (int k = 0; k < want; ++k) {
-    if (fscanf(fid, "%lf", &para[k]) != 1) {
-      fclose(fid);
-      delete p;
-      set_error("Reading error for Tersoff-1989 potential.");
-      return B200MD_ERR_ARG;
-    }
-  }
-  fclose(fid);
-  B2TersoffView& P = p->view;
-  std::memset(&P, 0, sizeof P);
-  fill(P.p[0], para);
-  p->rc = P.p[0].r2;
-  if (nt == 2) { // mixing rules, tersoff1989.cu:100-130
-    fill(P.p[1], para + 11);
-    const double chi = para[22];
-    B2TersoffPara& m = P.p[2];
-    m.a = std::sqrt(P.p[0].a * P.p[1].a);
-    m.b = std::sqrt(P.p[0].b * P.p[1].b) * chi;
-    m.lambda = 0.5 * (P.p[0].lambda + P.p[1].lambda);
-    m.mu = 0.5 * (P.p[0].mu + P.p[1].mu);
-    m.r1 = std::sqrt(P.p[0].r1 * P.p[1].r1);
-    m.r2 = std::sqrt(P.p[0].r2 * P.p[1].r2);
-    m.pi_factor = 3.14159265358979 / (m.r2 - m.r1);
-    p->rc = P.p[0].r2 > P.p[1].r2 ? P.p[0].r2 : P.p[1].r2;
-  } else {
-    P.p[1] = P.p[0];
-    P.p[2] = P.p[0];
-  }
-  P.rc2 = (float)(p->rc * p->rc);
+  p->nt = file.nt;
+  p->symbols = file.symbols;
+  p->rc = file.rc;
   p->n = num_atoms;
   const size_t N = (size_t)num_atoms;
-  // neighbor.initialize(rc, num_atoms, 50), tersoff1989.cu:149
-  const double rs = p->rc + 1.0;
-  const int mn_skin = (int)(50 * rs * rs * rs / (p->rc * p->rc * p->rc));
-  int rc = p->nb.init(num_atoms, p->rc, mn_skin);
+  int rc = p->nb.init(num_atoms, p->rc, file.mn_skin);
   if (rc != B200MD_OK) {
     delete p;
     return rc;
@@ -178,6 +108,8 @@ int b200md_tersoff_create(const char* path, int num_atoms, b200md_tersoff** out)
     set_error("out of device memory");
     return B200MD_ERR_CUDA;
   }
+  B2TersoffView& P = p->view;
+  P = file.view;
   P.n = num_atoms;
   P.atoms = p->nb.atoms.p;
   P.nn_skin = p->nb.nn_skin.p;

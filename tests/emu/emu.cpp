@@ -7,56 +7,21 @@
 // __graft_entry__.py or the gpumd_b200 package.  The block-cooperative pieces of the real kernels
 // (scan, shared-memory tile sort, atomics, warp reductions) are replaced by serial loops here
 // and are therefore covered only by the `-m gpu` tests.
-#include "../../gpumd_b200/csrc/b2_common.cuh"
-#include "../../gpumd_b200/csrc/b2_eam.cuh"
 #include "../../gpumd_b200/csrc/b2_bdp.cuh"
 #include "../../gpumd_b200/csrc/b2_integrate.cuh"
 #include "../../gpumd_b200/csrc/b2_lj.cuh"
 #include "../../gpumd_b200/csrc/b2_neighbor.cuh"
-#include "../../gpumd_b200/csrc/b2_nep.cuh"
-#include "../../gpumd_b200/csrc/b2_nep_model.h"
-#include "../../gpumd_b200/csrc/b2_tersoff.cuh"
+#include "../../gpumd_b200/csrc/b2_setup.h" // the library's own host setup
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
 
-namespace {
+using namespace b2;
 
-B2Box make_box(const double h[9], const int pbc[3])
-{
-  B2Box b;
-  double* c = b.h;
-  for (int d = 0; d < 9; ++d)
-    c[d] = h[d];
-  for (int d = 0; d < 3; ++d)
-    b.pbc[d] = pbc[d] ? 1 : 0;
-  c[9] = c[4] * c[8] - c[5] * c[7];
-  c[10] = c[2] * c[7] - c[1] * c[8];
-  c[11] = c[1] * c[5] - c[2] * c[4];
-  c[12] = c[5] * c[6] - c[3] * c[8];
-  c[13] = c[0] * c[8] - c[2] * c[6];
-  c[14] = c[2] * c[3] - c[0] * c[5];
-  c[15] = c[3] * c[7] - c[4] * c[6];
-  c[16] = c[1] * c[6] - c[0] * c[7];
-  c[17] = c[0] * c[4] - c[1] * c[3];
-  const double det = c[0] * c[9] + c[1] * c[12] + c[2] * c[15];
-  for (int d = 9; d < 18; ++d)
-    c[d] /= det;
-  b.volume = std::fabs(det);
-  for (int d = 0; d < 3; ++d) {
-    const int p = (d + 1) % 3, q = (d + 2) % 3;
-    const double u[3] = {c[p], c[p + 3], c[p + 6]}, w[3] = {c[q], c[q + 3], c[q + 6]};
-    const double s0 = u[1] * w[2] - u[2] * w[1], s1 = u[2] * w[0] - u[0] * w[2],
-                 s2 = u[0] * w[1] - u[1] * w[0];
-    b.thickness[d] = b.volume / std::sqrt(s0 * s0 + s1 * s1 + s2 * s2);
-  }
-  b.ortho = c[1] == 0 && c[2] == 0 && c[3] == 0 && c[5] == 0 && c[6] == 0 && c[7] == 0;
-  for (int d = 0; d < 18; ++d)
-    b.hf[d] = (float)c[d];
-  return b;
-}
+namespace {
 
 struct EmuNeighbor {
   int n = 0, mn_skin = 0;
@@ -95,16 +60,10 @@ struct EmuNeighbor {
   }
   int update(const B2Box& box, const int* type, const double* pos)
   {
-    for (int d = 0; d < 3; ++d)
-      if (box.pbc[d] && box.thickness[d] <= 2.5 * (rc + skin))
-        return 4;
-    B2Grid g;
-    for (int d = 0; d < 3; ++d) {
-      int nb = (int)std::floor(box.thickness[d] / (0.5 * (rc + skin)));
-      g.nb[d] = nb < 1 ? 1 : nb;
-      g.scale[d] = g.nb[d];
-    }
-    g.ncell = g.nb[0] * g.nb[1] * g.nb[2];
+    int reps[3];
+    const B2Grid g = make_grid(box, 0.5 * (rc + skin));
+    if (supercell_reps(box, rc, skin, reps) > 1 || grid_too_coarse(box, g))
+      return 4; // B200MD_ERR_SMALL_BOX, Neighbor::update
     cell_count.assign(g.ncell, 0);
     cell_fill.assign(g.ncell, 0);
     cell_start.assign(g.ncell + 1, 0);
@@ -169,7 +128,7 @@ std::string g_err;
 } // namespace
 
 struct emu_nep {
-  b2::NepModel m;
+  NepModel m;
   EmuNeighbor nb;
   int n = 0;
   std::vector<int> nn_r, nl_r, nn_a, nl_a;
@@ -178,8 +137,7 @@ struct emu_nep {
   std::vector<int> zbl_z;
   std::vector<float> cov;
   B2NepView P;
-  bool team = false, fuse_split = false; // same choices as nep_setup() in b2_nep.cu
-  bool rev_slot = false;
+  NepPlan plan;
   std::vector<int> aslot, nla_rs;
   int n_cell = 0;                        // atoms of the caller's cell (n > n_cell: supercell)
   int overwrite = 0, n_own = 0;          // b200md_nep_set_accumulate(p, 0) / set_owned requests
@@ -189,34 +147,23 @@ template <int K1>
 static void run_desc_radial(emu_nep* p, const B2Box& box)
 {
   std::vector<float> scratch((size_t)p->m.nt * K1 + 1);
-  if (!p->team && p->m.nt > 2 && !p->fuse_split)
+  if (!p->plan.team && p->m.nt > 2 && !p->plan.fuse_split)
     for (int i = 0; i < p->n; ++i)
       b2_body_split(i, p->P, box);
   for (int i = 0; i < p->n; ++i) {
-    if (p->team && p->m.nt == 1)
+    if (p->plan.team && p->m.nt == 1)
       b2_team_desc_radial<1, K1>(i, 0, p->P, box);
-    else if (p->team)
+    else if (p->plan.team)
       b2_team_desc_radial<2, K1>(i, 0, p->P, box);
     else if (p->m.nt == 1)
       b2_body_desc_radial<1, K1, true>(i, p->P, box, scratch.data(), 1, 0);
     else if (p->m.nt == 2)
       b2_body_desc_radial<2, K1, true>(i, p->P, box, scratch.data(), 1, 0);
     else {
-      // the library's choice (dispatch_desc_radial): register accumulators for 3..16 types
-      const char* e = getenv("B200MD_NEP_RADREG");
-      const int nt = p->m.nt;
-      int ntb = !(e && e[0] == '1') ? 0 : nt <= 4 ? 4 : nt <= 8 ? 8 : nt <= 16 ? 16 : 0;
-      if (ntb * K1 > 160)
-        ntb = 0;
-      {
-        // nep_setup()'s rule: the per-pair contraction when the shared-memory accumulators get too big
-        const char* d = getenv("B200MD_NEP_RADDIRECT");
-        if ((d && d[0] == '1') || (size_t)nt * K1 * 128 * sizeof(float) > 96 * 1024)
-          ntb = -1;
-      }
+      const int ntb = p->plan.rad_nt; // the k_desc_radial instance of dispatch_desc_radial
 #define EMU_DR(NT_)                                                                         \
   do {                                                                                      \
-    if (p->fuse_split)                                                                      \
+    if (p->plan.fuse_split)                                                                 \
       b2_body_desc_radial<NT_, K1, true>(i, p->P, box, scratch.data(), 1, 0);               \
     else                                                                                    \
       b2_body_desc_radial<NT_, K1, false>(i, p->P, box, scratch.data(), 1, 0);              \
@@ -239,9 +186,9 @@ template <int K1>
 static void run_force_final(emu_nep* p, const B2Box& box, double* pe, double* f, double* v)
 {
   for (int i = 0; i < p->n; ++i) {
-    if (p->team && p->m.nt == 1)
+    if (p->plan.team && p->m.nt == 1)
       b2_team_force_final<1, K1>(i, 0, p->P, box, pe, f, v);
-    else if (p->team)
+    else if (p->plan.team)
       b2_team_force_final<2, K1>(i, 0, p->P, box, pe, f, v);
     else if (p->m.nt == 1)
       b2_body_force_final<1, K1>(i, p->P, box, pe, f, v);
@@ -273,30 +220,26 @@ extern "C" {
 
 const char* emu_last_error(void) { return g_err.c_str(); }
 
-// (re)size every per-atom buffer for n atoms and point the view at them (nep_setup's host twin)
-static void emu_nep_alloc(emu_nep* p, int n)
+// plan, (re)size every per-atom buffer for n atoms and point the view at them (nep_setup's host twin);
+// returns the plan's error
+static std::string emu_nep_alloc(emu_nep* p, int n)
 {
-  b2::NepModel& m = p->m;
+  NepModel& m = p->m;
+  const std::string err = nep_plan(m, n, p->plan);
+  if (!err.empty())
+    return err;
+  const NepPlan& plan = p->plan;
   p->n = n;
   const size_t N = n;
-  const double rc = m.rc_radial_max, rs = rc + 1.0;
-  const char* team_env = std::getenv("B200MD_NEP_TEAM");
-  p->team = m.nt <= 2 && team_env && std::strcmp(team_env, "1") == 0;
-  p->fuse_split = rs * rs * rs / (rc * rc * rc) < 1.45;
-  p->nb.row_major = p->team;
-  {
-    const char* e = std::getenv("B200MD_NEP_REVSLOT");
-    p->rev_slot = m.nt > 2 && !p->team && !p->fuse_split && e && e[0] == '1';
-    p->nb.reverse = p->rev_slot;
-  }
-  p->nb.init(n, rc, (int)(m.MN_radial * rs * rs * rs / (rc * rc * rc)));
-  if (p->rev_slot) {
+  p->nb.row_major = plan.team;
+  p->nb.reverse = plan.rev_slot;
+  p->nb.init(n, m.rc_radial_max, plan.mn_skin);
+  if (plan.rev_slot) {
     p->aslot.assign((size_t)p->nb.pitch() * n, -1);
     p->nla_rs.assign(N * m.MN_angular, 0);
   }
-  const int pitch_r = (m.MN_radial + 7) / 8 * 8;
   p->nn_r.resize(N);
-  p->nl_r.resize(N * pitch_r);
+  p->nl_r.resize(N * plan.pitch_r);
   p->nn_a.resize(N);
   p->nl_a.resize(N * m.MN_angular);
   p->q.resize(N * m.dim);
@@ -307,53 +250,49 @@ static void emu_nep_alloc(emu_nep* p, int n)
   p->f12.resize(N * 3 * m.MN_angular + 1);
   p->acc.resize(N * 13);
   p->zbl_z = m.atomic_numbers;
-  p->cov.assign(b2::COVALENT_RADIUS, b2::COVALENT_RADIUS + 94);
+  p->cov.assign(COVALENT_RADIUS, COVALENT_RADIUS + 94);
   if (m.zbl_para.empty())
     m.zbl_para.push_back(0.0f);
   B2NepView& P = p->P;
-  std::memset(&P, 0, sizeof P);
-  P.nt = m.nt; P.nr1 = m.nr1; P.na1 = m.na1; P.kr1 = m.kr1; P.ka1 = m.ka1;
-  P.K1R = m.K1R; P.K1A = m.K1A; P.KP = m.KP; P.UST = m.UST;
-  P.has222 = m.has222; P.has1111 = m.has1111; P.num_L = m.num_L;
-  P.dim = m.dim; P.dim_ang = m.dim_angular; P.nneu = m.nneu; P.DIMP = m.DIMP;
-  P.zbl_enabled = m.zbl_enabled; P.zbl_flexible = m.zbl_flexible; P.zbl_typewise = m.zbl_typewise;
-  P.zbl_rc_inner = m.zbl_rc_inner; P.zbl_rc_outer = m.zbl_rc_outer;
-  P.zbl_typewise_factor = m.zbl_typewise_factor;
+  P = nep_view(m, plan, n);
   P.rc_r = m.rc_r.data(); P.rcinv_r = m.rcinv_r.data(); P.rc2_r = m.rc2_r.data();
   P.rc_a = m.rc_a.data(); P.rcinv_a = m.rcinv_a.data(); P.rc2_a = m.rc2_a.data();
-  {
-    const char* e = getenv("B200MD_NEP_CVEC");
-    const bool cvec = !(e && e[0] == '0');
-    P.c_a4 = reinterpret_cast<const float4*>(m.c_a4.data());
-    const char* d = getenv("B200MD_NEP_RADDIRECT");
-    const bool direct = m.nt > 2 && ((d && d[0] == '1') || (size_t)m.nt * m.K1R * 128 * sizeof(float) > 96 * 1024);
-    P.c_r4 = (cvec || direct) ? reinterpret_cast<const float4*>(m.c_r4.data()) : nullptr;
-    P.nqr = m.nqr;
-  }
+  P.c_a4 = reinterpret_cast<const float4*>(m.c_a4.data());
+  P.c_r4 = plan.c_r4 ? reinterpret_cast<const float4*>(m.c_r4.data()) : nullptr;
   P.c_r = m.c_r.data(); P.c_a = m.c_a.data(); P.w0p = m.w0p.data(); P.b0 = m.b0.data();
   P.w1 = m.w1.data(); P.bias = m.bias.data(); P.q_scaler = m.q_scaler.data();
   P.zbl_z = p->zbl_z.data(); P.zbl_para = m.zbl_para.data(); P.cov_radius = p->cov.data();
-  P.n = n; P.mn_r = m.MN_radial; P.mn_a = m.MN_angular;
   P.nn_r = p->nn_r.data(); P.nl_r = p->nl_r.data(); P.nn_a = p->nn_a.data(); P.nl_a = p->nl_a.data();
-  P.aslot = p->rev_slot ? p->aslot.data() : nullptr;
-  P.nla_rs = p->rev_slot ? p->nla_rs.data() : nullptr;
+  P.aslot = plan.rev_slot ? p->aslot.data() : nullptr;
+  P.nla_rs = plan.rev_slot ? p->nla_rs.data() : nullptr;
   P.q = p->q.data(); P.sfx = p->sfx.data(); P.FpR = p->FpR.data(); P.FpA = p->FpA.data(); P.U = p->U.data();
   P.f12 = p->f12.data(); P.acc = p->acc.data();
-  P.team = p->team ? 1 : 0;
-  P.pitch_r = pitch_r;
+  return "";
 }
 
 emu_nep* emu_nep_create(const char* path, int n)
 {
   emu_nep* p = new emu_nep;
   g_err = p->m.load(path);
+  if (g_err.empty())
+    g_err = emu_nep_alloc(p, n);
   if (!g_err.empty()) {
     delete p;
     return nullptr;
   }
   p->n_cell = n;
-  emu_nep_alloc(p, n);
   return p;
+}
+
+// the plan of the handle's last setup, in the order of emu_py.NEP_PLAN
+void emu_nep_plan(const emu_nep* p, long long* out)
+{
+  const NepPlan& q = p->plan;
+  const long long v[] = {q.mn_skin, q.pitch_r, q.team, q.fuse_split, q.radial_v2, q.sched, q.ang_fused,
+                         q.fused_shape, (long long)q.fused_smem, q.use_tc, q.utable_tc, q.rev_slot, q.slot_map,
+                         q.rad_reg, q.rad_direct, q.rad_nt, q.c_r4, q.ang_cstage, q.variant, q.tc_ctas_cap,
+                         q.debug_skip, q.ang_block, (long long)q.ang_smem, (long long)q.rad_smem};
+  std::copy(std::begin(v), std::end(v), out);
 }
 
 void emu_nep_destroy(emu_nep* p) { delete p; }
@@ -373,22 +312,18 @@ int emu_nep_compute(
     return 1;
   B2Box box = make_box(h, pbc);
   // small periodic boxes: supercell replication, the host twin of b200md_nep_compute
-  int reps[3] = {1, 1, 1};
-  const double need = 2.5 * (p->nb.rc + p->nb.skin);
-  for (int d = 0; d < 3; ++d)
-    if (box.pbc[d] && box.thickness[d] <= need)
-      reps[d] = (int)std::floor(need / box.thickness[d]) + 1;
-  const int R = reps[0] * reps[1] * reps[2];
+  int reps[3];
+  const int R = (int)supercell_reps(box, p->nb.rc, p->nb.skin, reps);
   if (R == 1) {
-    if (p->n != n)
-      emu_nep_alloc(p, n);
+    if (p->n != n && !(g_err = emu_nep_alloc(p, n)).empty())
+      return 1;
     p->P.overwrite = p->overwrite;
     p->P.n_own = p->n_own;
     return emu_nep_pipeline(p, box, type, pos, pe, force, virial);
   }
   const int nR = n * R;
-  if (p->n != nR)
-    emu_nep_alloc(p, nR);
+  if (p->n != nR && !(g_err = emu_nep_alloc(p, nR)).empty())
+    return 1;
   p->P.overwrite = p->overwrite;
   p->P.n_own = p->n_own;
   std::vector<int> t2(nR);
@@ -445,7 +380,7 @@ static int emu_nep_pipeline(
   P.perm = p->nb.perm.data();
   P.nn_skin = p->nb.nn_skin.data();
   P.nl_skin = p->nb.nl_skin.data();
-  P.rskin = p->rev_slot ? p->nb.rskin.data() : nullptr;
+  P.rskin = p->plan.rev_slot ? p->nb.rskin.data() : nullptr;
   P.skin_si = p->nb.v.skin_si;
   P.skin_sk = p->nb.v.skin_sk;
   P.flags = p->nb.flags.data();
@@ -471,11 +406,11 @@ static int emu_nep_pipeline(
   }
   for (int i = 0; i < n; ++i) {
     if (p->m.K1R == 9)
-      p->team ? b2_body_utable_planes<9>(i, P) : b2_body_utable<9>(i, P);
+      p->plan.team ? b2_body_utable_planes<9>(i, P) : b2_body_utable<9>(i, P);
     else if (p->m.K1R == 13)
-      p->team ? b2_body_utable_planes<13>(i, P) : b2_body_utable<13>(i, P);
+      p->plan.team ? b2_body_utable_planes<13>(i, P) : b2_body_utable<13>(i, P);
     else
-      p->team ? b2_body_utable_planes<17>(i, P) : b2_body_utable<17>(i, P);
+      p->plan.team ? b2_body_utable_planes<17>(i, P) : b2_body_utable<17>(i, P);
   }
   switch (p->m.K1A) {
     case 9: run_angular<9>(p, box, true); break;
@@ -520,7 +455,7 @@ void emu_nep_export_neighbors(
 {
   export_list(
     p->n, p->n_cell, p->P.perm, p->nn_r.data(), p->nl_r.data(),
-    p->team ? (size_t)p->P.pitch_r : 1, p->team ? 1 : (size_t)p->n, mn_r, NN_r, NL_r);
+    p->plan.team ? (size_t)p->P.pitch_r : 1, p->plan.team ? 1 : (size_t)p->n, mn_r, NN_r, NL_r);
   export_list(
     p->n, p->n_cell, p->P.perm, p->nn_a.data(), p->nl_a.data(), 1, (size_t)p->n, mn_a, NN_a, NL_a);
 }
@@ -543,29 +478,20 @@ void emu_nep_export_skin(emu_nep* p, int mn, int* NN, int* NL)
 
 // ---- LJ -------------------------------------------------------------------------------------
 struct emu_lj {
-  int nt, n;
-  double rc;
-  std::vector<float> s6, s12, c2;
+  LjFile file;
   EmuNeighbor nb;
   std::vector<double> acc;
 };
 
-emu_lj* emu_lj_create(int nt, const double* para, int n)
+emu_lj* emu_lj_create(const char* path, int n)
 {
   emu_lj* p = new emu_lj;
-  p->nt = nt;
-  p->n = n;
-  p->rc = 0;
-  for (int a = 0; a < nt * nt; ++a) {
-    const double eps = para[a * 3], sig = para[a * 3 + 1], cut = para[a * 3 + 2];
-    p->s6.push_back((float)(std::pow(sig, 6.0) * eps * 4.0));
-    p->s12.push_back((float)(std::pow(sig, 12.0) * eps * 4.0));
-    p->c2.push_back((float)(cut * cut));
-    if (p->rc < cut)
-      p->rc = cut;
+  g_err = load_lj(path, p->file);
+  if (!g_err.empty()) {
+    delete p;
+    return nullptr;
   }
-  const double rs = p->rc + 1.0;
-  p->nb.init(n, p->rc, (int)(4.19 * rs * rs * rs * 0.06) + 32);
+  p->nb.init(n, p->file.rc, p->file.mn_skin);
   p->acc.resize((size_t)13 * n);
   return p;
 }
@@ -580,10 +506,10 @@ int emu_lj_compute(
   if (rc)
     return rc;
   B2LjView P;
-  P.nt = p->nt;
-  P.s6e4 = p->s6.data();
-  P.s12e4 = p->s12.data();
-  P.rc2 = p->c2.data();
+  P.nt = p->file.nt;
+  P.s6e4 = p->file.s6e4.data();
+  P.s12e4 = p->file.s12e4.data();
+  P.rc2 = p->file.rc2.data();
   P.n = n;
   P.atoms = p->nb.atoms.data();
   P.nn_skin = p->nb.nn_skin.data();
@@ -598,50 +524,23 @@ int emu_lj_compute(
 
 // ---- Tersoff --------------------------------------------------------------------------------
 struct emu_tersoff {
-  int nt, n;
-  double rc;
   B2TersoffView P;
   EmuNeighbor nb;
   std::vector<int> nn, nl;
   std::vector<double> f12, acc;
 };
 
-static void ters_fill(B2TersoffPara& t, const double* p)
-{
-  t.a = p[0]; t.b = p[1]; t.lambda = p[2]; t.mu = p[3]; t.beta = p[4]; t.n = p[5];
-  t.c2 = p[6] * p[6]; t.d2 = p[7] * p[7]; t.h = p[8]; t.r1 = p[9]; t.r2 = p[10];
-  t.one_plus = 1.0 + t.c2 / t.d2;
-  t.pi_factor = 3.14159265358979 / (t.r2 - t.r1);
-  t.mhn = -0.5 / p[5];
-}
-
-emu_tersoff* emu_tersoff_create(int nt, const double* para, int n)
+emu_tersoff* emu_tersoff_create(const char* path, int n)
 {
   emu_tersoff* p = new emu_tersoff;
-  p->nt = nt;
-  p->n = n;
-  B2TersoffView& P = p->P;
-  std::memset(&P, 0, sizeof P);
-  ters_fill(P.p[0], para);
-  p->rc = P.p[0].r2;
-  if (nt == 2) {
-    ters_fill(P.p[1], para + 11);
-    B2TersoffPara& m = P.p[2];
-    m.a = std::sqrt(P.p[0].a * P.p[1].a);
-    m.b = std::sqrt(P.p[0].b * P.p[1].b) * para[22];
-    m.lambda = 0.5 * (P.p[0].lambda + P.p[1].lambda);
-    m.mu = 0.5 * (P.p[0].mu + P.p[1].mu);
-    m.r1 = std::sqrt(P.p[0].r1 * P.p[1].r1);
-    m.r2 = std::sqrt(P.p[0].r2 * P.p[1].r2);
-    m.pi_factor = 3.14159265358979 / (m.r2 - m.r1);
-    p->rc = P.p[0].r2 > P.p[1].r2 ? P.p[0].r2 : P.p[1].r2;
-  } else {
-    P.p[1] = P.p[0];
-    P.p[2] = P.p[0];
+  TersoffFile file;
+  g_err = load_tersoff(path, file);
+  if (!g_err.empty()) {
+    delete p;
+    return nullptr;
   }
-  P.rc2 = (float)(p->rc * p->rc);
-  const double rs = p->rc + 1.0;
-  p->nb.init(n, p->rc, (int)(50 * rs * rs * rs / (p->rc * p->rc * p->rc)));
+  p->P = file.view;
+  p->nb.init(n, file.rc, file.mn_skin);
   p->nn.resize(n);
   p->nl.resize((size_t)n * B2_TERSOFF_MAXL);
   p->f12.resize((size_t)3 * n * B2_TERSOFF_MAXL);
@@ -684,49 +583,21 @@ void emu_compute_heat(int n, const double* w, const double* v, double* heat)
 
 // ---- EAM ------------------------------------------------------------------------------------
 struct emu_eam {
-  int n;
-  B2EamView P;
-  std::vector<float> zp, Fp;
+  EamFile file;
+  std::vector<float> Fp;
   std::vector<double> acc;
   EmuNeighbor nb;
 };
 
-emu_eam* emu_eam_create(int model, int nt, const double* para, int n)
+emu_eam* emu_eam_create(const char* path, int n)
 {
   emu_eam* p = new emu_eam;
-  p->n = n;
-  B2EamView& P = p->P;
-  std::memset(&P, 0, sizeof P);
-  p->zp.assign((size_t)(nt > 0 ? nt : 1) * EZ_COUNT, 0.0f);
-  float rc = 0.0f;
-  if (model == 0) {
-    for (int t = 0; t < nt; ++t) {
-      float x[21];
-      for (int k = 0; k < 21; ++k)
-        x[k] = (float)para[t * 21 + k];
-      float* e = &p->zp[(size_t)t * EZ_COUNT];
-      e[EZ_RE_INV] = 1.0f / x[0]; e[EZ_FE] = x[1]; e[EZ_RHO_E_INV] = 1.0f / x[2];
-      e[EZ_RHO_S_INV] = 1.0f / x[3]; e[EZ_ALPHA] = x[4]; e[EZ_BETA] = x[5]; e[EZ_A] = x[6];
-      e[EZ_B] = x[7]; e[EZ_KAPPA] = x[8]; e[EZ_LAMBDA] = x[9]; e[EZ_FN0] = x[10]; e[EZ_FN1] = x[11];
-      e[EZ_FN2] = x[12]; e[EZ_FN3] = x[13]; e[EZ_F0] = x[14]; e[EZ_F1] = x[15]; e[EZ_F2] = x[16];
-      e[EZ_F3] = x[17]; e[EZ_ETA] = x[18]; e[EZ_FE_EMBED] = x[19]; e[EZ_RC] = x[20];
-      e[EZ_RHO_N] = x[2] * 0.85; e[EZ_RHO_0] = x[2] * 1.15; e[EZ_RHO_N_INV] = 1.0f / e[EZ_RHO_N];
-      if (rc < x[20])
-        rc = x[20];
-    }
-  } else {
-    float x[9];
-    for (int k = 0; k < 9; ++k)
-      x[k] = (float)para[k];
-    P.dA = x[0]; P.dd = x[1]; P.dc = x[2]; P.dc0 = x[3]; P.dc1 = x[4]; P.dc2 = x[5]; P.dc3 = x[6];
-    P.dc4 = x[7]; P.dB = x[8];
-    rc = P.dc > P.dd ? P.dc : P.dd;
+  g_err = load_eam(path, p->file);
+  if (!g_err.empty()) {
+    delete p;
+    return nullptr;
   }
-  P.model = model;
-  P.nt = nt;
-  P.rc = rc;
-  const double rs = rc + 1.0;
-  p->nb.init(n, rc, (int)(4.19 * rs * rs * rs * 0.2) + 32);
+  p->nb.init(n, p->file.rc, p->file.mn_skin);
   p->Fp.resize(n);
   p->acc.resize((size_t)13 * n);
   return p;
@@ -741,8 +612,8 @@ int emu_eam_compute(
   const int rc = p->nb.update(box, type, pos);
   if (rc)
     return rc;
-  B2EamView& P = p->P;
-  P.zp = p->zp.data();
+  B2EamView& P = p->file.view;
+  P.zp = p->file.zp.data();
   P.n = n;
   P.atoms = p->nb.atoms.data();
   P.nn_skin = p->nb.nn_skin.data();

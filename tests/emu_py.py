@@ -16,6 +16,12 @@ def _i(a):
     return a.ctypes.data_as(_ip)
 
 
+# NepPlan's fields in the order emu_nep_plan writes them
+NEP_PLAN = ("mn_skin", "pitch_r", "team", "fuse_split", "radial_v2", "sched", "ang_fused", "fused_shape", "fused_smem",
+            "use_tc", "utable_tc", "rev_slot", "slot_map", "rad_reg", "rad_direct", "rad_nt", "c_r4", "ang_cstage",
+            "variant", "tc_ctas_cap", "debug_skip", "ang_block", "ang_smem", "rad_smem")
+
+
 class EmuNep:
     def __init__(self, E, path, n):
         self.E = E
@@ -68,17 +74,28 @@ class EmuNep:
     def rebuilds(self):
         return self.E.emu_nep_rebuilds(self.h)
 
+    @property
+    def plan(self):
+        """the library's NepPlan for this model and atom count (b2_setup.h nep_plan)"""
+        v = (C.c_longlong * len(NEP_PLAN))()
+        self.E.emu_nep_plan(self.h, v)
+        return dict(zip(NEP_PLAN, v))
 
-class EmuLj:
-    def __init__(self, E, para, n):
+
+class EmuClassical:
+    """emu_{lj,tersoff,eam}_*: a potential file on n atoms"""
+
+    def __init__(self, E, kind, path, n):
         self.E = E
+        self.kind = kind
         self.n = n
-        para = np.ascontiguousarray(para, np.float64)
-        self.h = E.emu_lj_create(para.shape[0], _d(para.reshape(-1)), n)
+        self.h = getattr(E, f"emu_{kind}_create")(str(path).encode(), n)
+        if not self.h:
+            raise RuntimeError(E.emu_last_error().decode())
 
     def __del__(self):
         if getattr(self, "h", None):
-            self.E.emu_lj_destroy(self.h)
+            getattr(self.E, f"emu_{self.kind}_destroy")(self.h)
             self.h = None
 
     def compute(self, type_, h, pbc, pos):
@@ -88,53 +105,8 @@ class EmuLj:
         p = np.ascontiguousarray(pos, np.float64).reshape(-1)
         hh = np.ascontiguousarray(h, np.float64).reshape(9)
         pb = np.ascontiguousarray(pbc, np.int32)
-        rc = self.E.emu_lj_compute(self.h, n, _d(hh), _i(pb), _i(ty), _d(p), _d(pe), _d(f), _d(v))
-        return rc, dict(pe=pe, force=f.reshape(3, n), virial=v.reshape(9, n))
-
-
-class EmuTersoff:
-    def __init__(self, E, nt, para, n):
-        self.E = E
-        self.n = n
-        para = np.ascontiguousarray(para, np.float64)
-        self.h = E.emu_tersoff_create(nt, _d(para), n)
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            self.E.emu_tersoff_destroy(self.h)
-            self.h = None
-
-    def compute(self, type_, h, pbc, pos):
-        n = self.n
-        pe, f, v = np.zeros(n), np.zeros(3 * n), np.zeros(9 * n)
-        ty = np.ascontiguousarray(type_, np.int32)
-        p = np.ascontiguousarray(pos, np.float64).reshape(-1)
-        hh = np.ascontiguousarray(h, np.float64).reshape(9)
-        pb = np.ascontiguousarray(pbc, np.int32)
-        rc = self.E.emu_tersoff_compute(self.h, n, _d(hh), _i(pb), _i(ty), _d(p), _d(pe), _d(f), _d(v))
-        return rc, dict(pe=pe, force=f.reshape(3, n), virial=v.reshape(9, n))
-
-
-class EmuEam:
-    def __init__(self, E, model, nt, para, n):
-        self.E = E
-        self.n = n
-        para = np.ascontiguousarray(para, np.float64)
-        self.h = E.emu_eam_create(model, nt, _d(para), n)
-
-    def __del__(self):
-        if getattr(self, "h", None):
-            self.E.emu_eam_destroy(self.h)
-            self.h = None
-
-    def compute(self, type_, h, pbc, pos):
-        n = self.n
-        pe, f, v = np.zeros(n), np.zeros(3 * n), np.zeros(9 * n)
-        ty = np.ascontiguousarray(type_, np.int32)
-        p = np.ascontiguousarray(pos, np.float64).reshape(-1)
-        hh = np.ascontiguousarray(h, np.float64).reshape(9)
-        pb = np.ascontiguousarray(pbc, np.int32)
-        rc = self.E.emu_eam_compute(self.h, n, _d(hh), _i(pb), _i(ty), _d(p), _d(pe), _d(f), _d(v))
+        rc = getattr(self.E, f"emu_{self.kind}_compute")(self.h, n, _d(hh), _i(pb), _i(ty), _d(p), _d(pe), _d(f),
+                                                          _d(v))
         return rc, dict(pe=pe, force=f.reshape(3, n), virial=v.reshape(9, n))
 
 
@@ -153,18 +125,12 @@ class Emu:
         E.emu_nep_export_skin.argtypes = [C.c_void_p, C.c_int, _ip, _ip]
         E.emu_nep_export_descriptors.argtypes = [C.c_void_p, _fp]
         E.emu_nep_set_mode.argtypes = [C.c_void_p, C.c_int, C.c_int]
-        E.emu_lj_create.restype = C.c_void_p
-        E.emu_lj_create.argtypes = [C.c_int, _dp, C.c_int]
-        E.emu_lj_destroy.argtypes = [C.c_void_p]
-        E.emu_lj_compute.argtypes = [C.c_void_p, C.c_int, _dp, _ip, _ip, _dp, _dp, _dp, _dp]
-        E.emu_tersoff_create.restype = C.c_void_p
-        E.emu_tersoff_create.argtypes = [C.c_int, _dp, C.c_int]
-        E.emu_tersoff_destroy.argtypes = [C.c_void_p]
-        E.emu_tersoff_compute.argtypes = [C.c_void_p, C.c_int, _dp, _ip, _ip, _dp, _dp, _dp, _dp]
-        E.emu_eam_create.restype = C.c_void_p
-        E.emu_eam_create.argtypes = [C.c_int, C.c_int, _dp, C.c_int]
-        E.emu_eam_destroy.argtypes = [C.c_void_p]
-        E.emu_eam_compute.argtypes = [C.c_void_p, C.c_int, _dp, _ip, _ip, _dp, _dp, _dp, _dp]
+        E.emu_nep_plan.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
+        for k in ("lj", "tersoff", "eam"):
+            getattr(E, f"emu_{k}_create").restype = C.c_void_p
+            getattr(E, f"emu_{k}_create").argtypes = [C.c_char_p, C.c_int]
+            getattr(E, f"emu_{k}_destroy").argtypes = [C.c_void_p]
+            getattr(E, f"emu_{k}_compute").argtypes = [C.c_void_p, C.c_int, _dp, _ip, _ip, _dp, _dp, _dp, _dp]
         E.emu_compute_heat.argtypes = [C.c_int, _dp, _dp, _dp]
         E.emu_apply_pbc.argtypes = [C.c_int, _dp, _ip, _dp]
         E.emu_velocity_verlet.argtypes = [C.c_int, C.c_int, C.c_double, _dp, _dp, _dp, _dp]
@@ -183,14 +149,14 @@ class Emu:
     def nep(self, path, n):
         return EmuNep(self.E, path, n)
 
-    def lj(self, para, n):
-        return EmuLj(self.E, para, n)
+    def lj(self, path, n):
+        return EmuClassical(self.E, "lj", path, n)
 
-    def tersoff(self, nt, para, n):
-        return EmuTersoff(self.E, nt, para, n)
+    def tersoff(self, path, n):
+        return EmuClassical(self.E, "tersoff", path, n)
 
-    def eam(self, model, nt, para, n):
-        return EmuEam(self.E, model, nt, para, n)
+    def eam(self, path, n):
+        return EmuClassical(self.E, "eam", path, n)
 
     def compute_heat(self, virial, vel):
         n = vel.shape[1]

@@ -120,14 +120,7 @@ def test_oracle_matches_fp64_reference(oracle, case):
 # ---------------------------------------------------------------- host build of the kernel bodies
 
 def emu_handle(emu, kind, path, n):
-    from oracle import oracle_py
-    if kind == "lj":
-        return emu.lj(cc.lj_table(path), n)
-    if kind == "tersoff":
-        nt, p = oracle_py.tersoff_parameters(path)
-        return emu.tersoff(nt, p, n)
-    model, nt, p = oracle_py.eam_parameters(path)
-    return emu.eam(model, nt, p, n)
+    return getattr(emu, kind)(path, n)
 
 
 def check_vs_oracle(out, r, n, kind, path):

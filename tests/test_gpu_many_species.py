@@ -15,7 +15,7 @@ from gpumd_b200.structures import fcc
 from test_gpu_nep_modes import _call
 from test_gpu_nep_species import MLP_MODELS, _env, check_mlp, check_tile_rule, load_ann
 from test_gpu_parity import GpuNep, eng  # noqa: F401  (module fixture: the library, built)
-from test_many_species_cpu import BOXES, MANY_SPECIES_CASES, check_case
+from test_many_species_cpu import BOXES, MANY_SPECIES_CASES, RADREG_NT, check_case
 
 pytestmark = pytest.mark.gpu
 
@@ -33,8 +33,6 @@ EXPECT = {
     "16sp_k13": dict(ang_block=128, radial_nt=-1, split=0, cstage=0, dimp=32, tc=1, tc3=1),
     "8sp_wide": dict(ang_block=64, radial_nt=0, split=1, cstage=1, dimp=128, tc=0, tc3=0),
 }
-# B200MD_NEP_RADREG=1: NT of the register-accumulator instance (NT * K1 <= 160 registers)
-RADREG_NT = {"3sp_nep5_flexzbl": 4, "5sp_zbl_k17_rc8": 8, "3sp_namax17": 4, "8sp_wide": 8}
 
 
 def expected(case, mlp, **over):

@@ -262,24 +262,37 @@ def test_reference_goldens_directly(emu):
     check_reference_goldens(lambda model, n: emu.nep(GOLDEN / model, n), assert_close, TOL)
 
 
-def test_lj_bodies_match_oracle(oracle, emu):
+def write_potential(path, head, rows):
+    """A potential file: the first line, then one line per row of numbers (repr: the values round-trip)."""
+    path.write_text("\n".join([head] + [" ".join(repr(float(x)) for x in r) for r in rows]) + "\n")
+    return path
+
+
+def write_lj(path, para, symbols):
+    """An `lj` file of the table para[a][b] = (epsilon, sigma, cutoff)."""
+    nt = para.shape[0]
+    return write_potential(path, f"lj {nt} {' '.join(symbols)}", para.reshape(nt * nt, 3))
+
+
+def test_lj_bodies_match_oracle(oracle, emu, tmp_path):
     s = fcc(6, 5.30, rattle=0.1, seed=2)  # 31.8 A box > 2.5*(10+1)
     n = s["type"].shape[0]
     para = np.array([[[1.032e-2, 3.405, 10.0]]])
     r = oracle.lj_compute(para, s["type"], s["h"], s["pbc"], s["pos"])
-    rc, out = emu.lj(para, n).compute(s["type"], s["h"], s["pbc"], s["pos"])
+    rc, out = emu.lj(write_lj(tmp_path / "lj.txt", para, ["Ar"]), n).compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc == 0
     assert_close(out["pe"], r["pe"], rtol=1e-5, atol=1e-7, what="pe")
     assert_close(out["force"], r["force"], **TOL["force"], what="force")
     assert_close(out["virial"], r["virial"], **TOL["virial"], what="virial")
 
 
-def test_lj_two_types(oracle, emu):
+def test_lj_two_types(oracle, emu, tmp_path):
     s = fcc(6, 5.30, rattle=0.1, seed=9, num_types=2, symbols=("Ar", "Ar"))
     n = s["type"].shape[0]
     para = np.array([[[1.0e-2, 3.4, 10.0], [0.8e-2, 3.2, 9.0]], [[0.8e-2, 3.2, 9.0], [1.2e-2, 3.0, 8.0]]])
     r = oracle.lj_compute(para, s["type"], s["h"], s["pbc"], s["pos"])
-    rc, out = emu.lj(para, n).compute(s["type"], s["h"], s["pbc"], s["pos"])
+    path = write_lj(tmp_path / "lj.txt", para, ["Ar", "Ar"])
+    rc, out = emu.lj(path, n).compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc == 0
     assert_close(out["force"], r["force"], **TOL["force"], what="force")
     assert_close(out["pe"], r["pe"], rtol=1e-5, atol=1e-7, what="pe")
@@ -316,23 +329,25 @@ def test_integrate_bodies(oracle, emu):
 
 
 @pytest.mark.parametrize("case", ["Si", "SiC_like"])
-def test_tersoff_bodies_match_oracle(oracle, emu, case):
+def test_tersoff_bodies_match_oracle(oracle, emu, case, tmp_path):
     """Tersoff-1989 is FP64 end to end in the reference; our fused kernel only re-orders the
     arithmetic (radial functions evaluated once per neighbour), so agreement is at 1e-10."""
     from gpumd_b200.structures import diamond
+    path = GOLDEN / "tersoff_Si_1989.txt"
     if case == "Si":
-        nt, para = oracle.tersoff_parameters(GOLDEN / "tersoff_Si_1989.txt")
+        nt, para = oracle.tersoff_parameters(path)
         s = diamond(4, a=5.431, rattle=0.08, seed=12)  # 512 atoms, 21.7 A box
         types = s["type"]
     else:  # two types: Si parameters twice with perturbed second set and chi != 1 (mixing rules)
-        _, p0 = oracle.tersoff_parameters(GOLDEN / "tersoff_Si_1989.txt")
+        _, p0 = oracle.tersoff_parameters(path)
         p1 = p0 * np.array([1.05, 0.97, 1.02, 0.98, 1.0, 1.0, 1.0, 1.0, 1.0, 0.98, 0.99])
         nt, para = 2, np.concatenate([p0, p1, [0.9776]])
+        path = write_potential(tmp_path / "tersoff.txt", "tersoff_1989 2 Si C", [p0, p1, [0.9776]])
         s = diamond(4, a=5.431, rattle=0.08, seed=13)
         types = (np.arange(s["type"].shape[0]) % 2).astype(np.int32)
     n = types.shape[0]
     r = oracle.tersoff_compute(nt, para, types, s["h"], s["pbc"], s["pos"])
-    rc, out = emu.tersoff(nt, para, n).compute(types, s["h"], s["pbc"], s["pos"])
+    rc, out = emu.tersoff(path, n).compute(types, s["h"], s["pbc"], s["pos"])
     assert rc == 0
     assert_close(out["pe"], r["pe"], rtol=1e-10, atol=1e-11, what="pe")
     assert_close(out["force"], r["force"], rtol=1e-9, atol=1e-10, what="force")
@@ -363,7 +378,7 @@ def test_eam_bodies_match_oracle(oracle, emu, potfile, ntypes):
     s = fcc(6, 3.615, rattle=0.08, seed=31, num_types=nt, symbols=["Cu", "Fe", "Ni"][:nt])
     n = s["type"].shape[0]  # 864 atoms, 21.7 A box (rc 6.5 / 4.3 A)
     r = oracle.eam_compute(model, nt, para, s["type"], s["h"], s["pbc"], s["pos"])
-    rc, out = emu.eam(model, nt, para, n).compute(s["type"], s["h"], s["pbc"], s["pos"])
+    rc, out = emu.eam(GOLDEN / potfile, n).compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc == 0
     assert_close(out["pe"], r["pe"], rtol=2e-6, atol=1e-6, what="pe")
     check_fv(out, r)

@@ -36,6 +36,9 @@ MANY_SPECIES_CASES = {
 
 BOXES = {"ortho": lambda s: s, "triclinic": shear, "slab": slab}
 
+# B200MD_NEP_RADREG=1: NT of the register-accumulator instance (NT * K1 <= 160 registers)
+RADREG_NT = {"3sp_nep5_flexzbl": 4, "5sp_zbl_k17_rc8": 8, "3sp_namax17": 4, "8sp_wide": 8}
+
 
 def check_case(oracle, dev, case, s):
     """check_nep on a case; the 8 A models (~300 radial neighbours) with the FP32 restatement's own distance

@@ -16,11 +16,11 @@ import pytest
 
 import cases_classical as cc
 from cases import NEP_CASES, shear
-from conftest import GOLDEN
+from conftest import GOLDEN, assert_close
 from gpumd_b200.structures import diamond, nep_type_order, rocksalt_pbte
 from test_classical_cpu import check_vs_fp64, check_vs_oracle, emu_handle
 from test_few_species_cpu import alloy
-from test_kernel_bodies_cpu import check_nep
+from test_kernel_bodies_cpu import check_fv, check_nep
 
 
 # ---------------------------------------------------------------- structures
@@ -389,22 +389,21 @@ def tersoff_shell(extra):
 def test_tersoff_angular_overflow_bodies(oracle, emu):
     """Tersoff's local list holds 32 neighbours: 33 latch B2_ERR_ANGULAR_OVERFLOW, 32 are legal and match the
     oracle."""
-    nt, p = oracle.tersoff_parameters(cc.SI)
     s = tersoff_shell(1)
     n = s["type"].shape[0]
-    dev = emu.tersoff(nt, p, n)
+    dev = emu.tersoff(cc.SI, n)
     rc, _ = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc != 0 and emu.E.emu_tersoff_error_bits(dev.h) == 4
     s = tersoff_shell(0)
     n = s["type"].shape[0]
-    dev = emu.tersoff(nt, p, n)
+    dev = emu.tersoff(cc.SI, n)
     rc, out = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
     assert rc == 0 and emu.E.emu_tersoff_error_bits(dev.h) == 0
     check_vs_oracle(out, cc.oracle32("tersoff", cc.SI, s), n, "tersoff", cc.SI)
 
 
 # LJ and EAM: the skin list is their only list.  Its capacity is k ((rc + 1) / rc)^3 entries, k = 700 (LJ) /
-# 400 (EAM) (b2_md.cu, b2_eam.cu), or with B200MD_TIGHT_LISTS=1 (and in the host build) what a sphere of
+# 400 (EAM) (b2_setup.h), or with B200MD_TIGHT_LISTS=1 what a sphere of
 # rc + 1 holds at 0.06 / 0.2 atoms per A^3, plus 32.  The shell then puts ~930 / ~620 (~370 / ~320) atoms
 # 0.5 A outside the cutoff of the centre: about one atom per 1.1 A^2 of the sphere at most, a finite, if
 # unphysical, density.
@@ -412,7 +411,7 @@ SKIN_POT = {"lj": (cc.LJ1, 700, 0.06), "eam": (GOLDEN / cc.EAM_FILES["cu_zhou"],
 
 
 def classical_skin_capacity(kind, tight):
-    """The expressions of b2_md.cu / b2_eam.cu (EAM holds its cutoff in float)."""
+    """The expressions of b2_setup.h (EAM holds its cutoff in float)."""
     path, k, dens = SKIN_POT[kind]
     rc = cc.cutoff(kind, path)
     if kind == "eam":
@@ -427,17 +426,27 @@ def skin_shell(kind, extra, tight):
 
 
 @pytest.mark.parametrize("kind", list(SKIN_POT))
-def test_classical_skin_overflow_bodies(oracle, emu, kind):
-    """count = capacity + 1 latches B2_ERR_SKIN_OVERFLOW; count = capacity is legal and matches the oracle (the
-    host build has the tight capacity)."""
+def test_classical_skin_overflow_bodies(oracle, emu, kind, monkeypatch):
+    """count = capacity + 1 latches B2_ERR_SKIN_OVERFLOW; count = capacity is legal and matches the oracle, for
+    the default and the B200MD_TIGHT_LISTS=1 capacity."""
     path = SKIN_POT[kind][0]
-    s = skin_shell(kind, 1, tight=True)
-    dev = emu_handle(emu, kind, path, s["type"].shape[0])
-    rc, _ = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
-    assert rc != 0 and getattr(emu.E, f"emu_{kind}_error_bits")(dev.h) == 1
-    s = skin_shell(kind, 0, tight=True)
-    n = s["type"].shape[0]
-    dev = emu_handle(emu, kind, path, n)
-    rc, out = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
-    assert rc == 0 and getattr(emu.E, f"emu_{kind}_error_bits")(dev.h) == 0
-    check_vs_oracle(out, cc.oracle32(kind, path, s), n, kind, path)
+    for tight in (False, True):
+        if tight:
+            monkeypatch.setenv("B200MD_TIGHT_LISTS", "1")
+        else:
+            monkeypatch.delenv("B200MD_TIGHT_LISTS", raising=False)
+        s = skin_shell(kind, 1, tight)
+        dev = emu_handle(emu, kind, path, s["type"].shape[0])
+        rc, _ = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
+        assert rc != 0 and getattr(emu.E, f"emu_{kind}_error_bits")(dev.h) == 1
+        s = skin_shell(kind, 0, tight)
+        n = s["type"].shape[0]
+        dev = emu_handle(emu, kind, path, n)
+        rc, out = dev.compute(s["type"], s["h"], s["pbc"], s["pos"])
+        assert rc == 0 and getattr(emu.E, f"emu_{kind}_error_bits")(dev.h) == 0
+        r = cc.oracle32(kind, path, s)
+        if tight:
+            check_vs_oracle(out, r, n, kind, path)
+        else:  # ~1.2 A apart: site energies of 1e4 - 1e5 eV, so only the relative parts of the tolerances apply
+            assert_close(out["pe"], r["pe"], rtol=1e-5, atol=1e-5, what="pe")
+            check_fv(out, r)
